@@ -119,6 +119,6 @@ def require_cuda():
     import torch
     lib()
     if not torch.cuda.is_available():
-        raise AnvError("anovos_b200 needs a CUDA device (sm_100a); torch.cuda.is_available() is False. "
+        raise AnvError("anovos_b200 needs a CUDA device (sm_90a); torch.cuda.is_available() is False. "
                        "There is no CPU fallback.")
     return torch

@@ -1,4 +1,4 @@
-"""Build libanovos_b200.so in-tree with nvcc for sm_100a (no GPU needed: nvcc cross-compiles).
+"""Build libanovos_b200.so in-tree with nvcc for sm_90a (H100; no GPU needed: nvcc cross-compiles).
 
     python -m anovos_b200.build            # incremental
     python -m anovos_b200.build --force
@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libanovos_b200.so")
 SOURCES = ["capi.cu", "scan_host.cu", "scan_mom.cu", "scan_hist.cu", "scan_fused.cu", "scan_assign.cu", "drift.cu", "synth.cu", "select.cu", "hll.cu", "sort.cu", "sample.cu", "gk_host.cu"]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ["-O3", "-std=c++17"] + GENCODE + ["-lineinfo",
               "--expt-relaxed-constexpr", "--expt-extended-lambda", "-Xcompiler", "-fPIC,-O3",
               "-Xptxas", "-v"]
 
@@ -56,7 +57,7 @@ def build_variant(tag, defines):
     if any(p.wait() != 0 for p in procs):
         raise RuntimeError("nvcc failed for variant " + tag)
     lib = os.path.join(HERE, "build", "variants", "libanovos_b200_%s.so" % tag)
-    subprocess.check_call([_nvcc(), "-shared", "-o", lib] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([_nvcc(), "-shared", "-o", lib] + objs + GENCODE)
     return lib
 
 
@@ -92,7 +93,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError("nvcc failed")
     if force or procs or _stale(LIB, objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + GENCODE
         subprocess.check_call(cmd)
     with open(stamp, "w") as f:
         f.write(digest)

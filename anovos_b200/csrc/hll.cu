@@ -137,7 +137,7 @@ extern "C" int anv_hll_registers(const anv_column_t* cols, int n_cols, int64_t n
   HllParams P{};
   P.cols = cols; P.n_cols = n_cols; P.n_rows = n_rows; P.p = p; P.regs = regs;
   P.use_smem = p <= 14;
-  int sms = 148, dev = 0;
+  int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   int64_t per_col = ((int64_t)sms * 4 + n_cols - 1) / n_cols;

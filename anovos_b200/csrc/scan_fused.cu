@@ -1,9 +1,7 @@
 // K1+K2 instantiation: moments and private-counter histogram in one read.
 // Two kernels, same results bit for bit: the register-staged loop (default) and the cp.async-staged loop (ANV_FUSED_STAGED=1:
-// null-free columns go through a thread-private shared-memory ring).  Measured on B200 (profiles/r2b_fused_ab.md): the ring
-// removes the long-scoreboard stalls (4.8 -> 0.9 per issue) and wins 2-9 % on null-free frames, but costs 8 % more
-// instructions; at the north-star configuration (3 of 4 numeric columns carry a bitmap, the SM clock under the power cap) the
-// register-staged loop is 1 % ahead, so it stays the default.
+// null-free columns go through a thread-private shared-memory ring).  The ring hides load latency behind the thread's own
+// next batches but costs more instructions per element; the register-staged loop is the default.
 #include <stdlib.h>
 #include "scan_impl.cuh"
 namespace anv {

@@ -42,7 +42,7 @@ __global__ void __launch_bounds__(32) finalize_moments(const Partial* partials, 
 
 int pick_tile_rows(int64_t n_rows, int n_cols) {
   // >= ~8 tiles per SM across the launch, tile in [16Ki, 256Ki] rows, multiple of 1024
-  int sms = 148, dev = 0;
+  int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   int64_t want_tiles = (int64_t)sms * 8;

@@ -51,8 +51,8 @@ struct ScanParams {
   uint32_t stage_off;
 };
 
-// Per-kernel tuning (measured on B200, scripts/tune.sh): 8 x 128-bit loads in flight per
-// thread and 4 CTAs of 256 threads per SM (<= 64 registers, no spills) win for every variant.
+// Per-kernel tuning (scripts/tune.sh sweeps ANV_UNROLL / ANV_MINBLOCKS): 8 x 128-bit loads in flight per thread and
+// 4 CTAs of 256 threads per SM (<= 64 registers).
 template <bool MOM, int HPATH, bool ASSIGN> struct Tune {
 #ifdef ANV_UNROLL
   static constexpr int U = ANV_UNROLL;
@@ -193,9 +193,10 @@ template <> __device__ __forceinline__ void count_nonzero<int32_t>(uint32_t& n, 
   asm("{\n\t.reg .pred p;\n\tsetp.ne.s32 p, %1, 0;\n\t@p add.u32 %0, %0, 1;\n\t}" : "+r"(n) : "r"(x));
 }
 
-// 3-input min / max (FMNMX3 / VIMNMX3 on sm_100a): one instruction per two elements.
-__device__ __forceinline__ float min3(float a, float b, float c) { float r; asm("min.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c)); return r; }
-__device__ __forceinline__ float max3(float a, float b, float c) { float r; asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c)); return r; }
+// 3-input min / max.  sm_90a has no 3-input FMNMX (the PTX form needs sm_100): two FMNMX for floats, one VIMNMX3
+// for int32.  fminf / fmaxf drop a NaN operand exactly as PTX min / max do.
+__device__ __forceinline__ float min3(float a, float b, float c) { return fminf(a, fminf(b, c)); }
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(a, fmaxf(b, c)); }
 __device__ __forceinline__ int32_t min3(int32_t a, int32_t b, int32_t c) { return __vimin3_s32(a, b, c); }
 __device__ __forceinline__ int32_t max3(int32_t a, int32_t b, int32_t c) { return __vimax3_s32(a, b, c); }
 __device__ __forceinline__ double min3(double a, double b, double c) { return fmin(a, fmin(b, c)); }
@@ -355,7 +356,7 @@ __device__ __forceinline__ void scan_tile(const ScanParams& P, const anv_column_
 #pragma unroll
       for (int i = 0; i < VEC; ++i) e[i] = ((vb >> (i + 1)) & 1u) ? e[i] : pivot_t;
     }
-    if (MOM) {  // two elements per FMNMX3 / VIMNMX3
+    if (MOM) {  // two elements per min3 / max3
 #pragma unroll
       for (int i = 0; i < VEC; i += 2) {
         mn = min3(mn, e[i], e[i + 1]);
@@ -696,7 +697,7 @@ static int launch_scan(ScanParams& P, size_t smem, cudaStream_t st) {
   if (STAGED) {  // the ring sits behind the counters, 16-byte aligned
     P.stage_off = (uint32_t)((smem + 15) & ~(size_t)15);
     smem = P.stage_off + STAGE_BYTES;
-    // four CTAs of (counters + ring) per SM need nearly all of the 228 KB: ask for the largest shared-memory carve-out
+    // four CTAs of (counters + ring) per SM need most of the 228 KB of an H100 SM: ask for the largest shared-memory carve-out
     ANV_CUDA(cudaFuncSetAttribute(scan_kernel<MOM, HPATH, ASSIGN, STAGED>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                   (int)cudaSharedmemCarveoutMaxShared));
   }

@@ -314,7 +314,7 @@ __global__ void __launch_bounds__(256) select_scan_kernel(SelState* state, unsig
 }
 
 static int sel_tile_rows(int64_t n_rows, int n_cols) {
-  int sms = 148, dev = 0;
+  int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   int64_t want = (int64_t)sms * 4;

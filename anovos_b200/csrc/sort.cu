@@ -391,31 +391,29 @@ __global__ void __launch_bounds__(ANV_BLOCK) sort_bases_kernel(const SortParams<
   }
 }
 
-// Lanes of `act` holding the same 8-bit digit.  Per bit: test, ballot of "my bit is set", and ONE three-input logic op
-// m &= ballot ^ (my bit ? 0 : ~0)  - keep the lanes whose bit equals mine (4 SASS instructions per bit + the select).
-#define ANV_PEER_BIT(B)                                                                                       \
-  asm volatile("{\n\t.reg .pred p;\n\t.reg .b32 t, bal, s;\n\tand.b32 t, %1, " #B ";\n\tsetp.ne.u32 p, t, 0;\n\t"     \
-               "vote.sync.ballot.b32 bal, p, 0xffffffff;\n\tselp.b32 s, 0, -1, p;\n\t"                               \
-               "lop3.b32 %0, %0, bal, s, 0x60;\n\t}"                                                          \
-               : "+r"(m) : "r"(d))
+// Lanes of `act` holding the same 8-bit digit.  Per bit: ballot of "my bit is set", keep the lanes whose bit equals mine
+// (m &= my bit ? ballot : ~ballot).  Written in C++: the same sequence as inline-asm blocks of vote.sync keeps ptxas for
+// sm_90a from finishing the scatter kernels.
 __device__ __forceinline__ uint32_t peers8(uint32_t d, uint32_t act) {
   uint32_t m = act;
-  ANV_PEER_BIT(1); ANV_PEER_BIT(2); ANV_PEER_BIT(4); ANV_PEER_BIT(8);
-  ANV_PEER_BIT(16); ANV_PEER_BIT(32); ANV_PEER_BIT(64); ANV_PEER_BIT(128);
+#pragma unroll
+  for (int b = 0; b < 8; ++b) {
+    const bool p = (d >> b) & 1u;
+    const uint32_t bal = __ballot_sync(ANV_FULL, p);
+    m &= p ? bal : ~bal;
+  }
   return m;
 }
-#undef ANV_PEER_BIT
 
 
 // ---- pass step 1: per-tile digit histogram ------------------------------------------------------
-// Plain shared-memory atomics (hardware handles same-address lanes far faster than a
-// match_any pre-aggregation: measured 4-5x on B200).
+// Plain shared-memory atomics (the hardware resolves same-address lanes itself; a match_any
+// pre-aggregation only adds instructions).
 #ifndef ANV_HIST_TPC
 #define ANV_HIST_TPC 4
 #endif
-// tiles per tile-histogram CTA.  Measured (c2 / c3 sort call, ms): 1 tile 11.36 / 317.3, 4 tiles 11.19 / 314.8 - the two dependent
-// loads that start a CTA (column state, then keys) are paid once per 64 KB.  The same knob on the scatter (2 tiles: 12.42 /
-// 354.6) and the run summaries (4 tiles: 11.29 / 316.8) does not pay and stays at 1.
+// tiles per tile-histogram CTA: the two dependent loads that start a CTA (column state, then keys) are paid once per 64 KB.
+// The same knob on the scatter and the run summaries stays at 1.
 constexpr int HIST_TPC = ANV_HIST_TPC;
 template <typename K>
 __global__ void __launch_bounds__(ANV_BLOCK) sort_hist_kernel(const SortParams<K> P) {
@@ -457,7 +455,7 @@ __global__ void __launch_bounds__(ANV_BLOCK) sort_hist_kernel(const SortParams<K
 
 // ---- pass step 2: exclusive scan of [256][n_tiles] per column + skip decision ------------------------------------
 // Two launches with one CTA per (digit, column) - 256 x n_cols CTAs instead of n_cols (a batch of 15-50 columns left most of
-// the 148 SMs idle while a single CTA per column walked 6 M entries at c3):
+// the SMs idle while a single CTA per column walked millions of entries):
 //   sort_totals_kernel   digit_total[c][d] = sum over tiles of tile_hist[c][d][*]
 //   sort_scan_kernel     base(d) = sum of the totals of the smaller digits (256 values, one warp scan per CTA), then the exclusive
 //                        scan of the digit's own tile counts on top of it; the CTA of digit 0 also takes the device-side
@@ -544,7 +542,7 @@ __global__ void __launch_bounds__(ANV_BLOCK) sort_scan_kernel(const SortParams<K
 
 // ---- pass step 3: stable scatter ---------------------------------------------------------------
 // Ranking: warp w owns 512 consecutive keys (16 rounds of 32); the lanes holding the same digit
-// are found with 8 ballots (cheaper than MATCH.ANY on sm_100a), all 16 rounds' loads and peer
+// are found with 8 ballots (instead of one MATCH.ANY), all 16 rounds' loads and peer
 // masks are computed up front (independent), then the warp-private digit counters are advanced
 // round by round.  The tile is then REORDERED IN SHARED MEMORY into digit order, so the global
 // writes are coalesced runs (full 32-byte sectors) instead of 4-byte scatters.
@@ -1040,9 +1038,8 @@ static int run_mode_distinct(const anv_column_t* cols, int n_cols, int64_t n_row
   if (hll_regs) ANV_CUDA(cudaMemsetAsync(hll_regs, 0, ((size_t)n_cols << hll_p) * sizeof(uint32_t), st));
   // Default: three kernels per pass (tile histogram, (digit, column)-parallel scan, stable scatter).  ANV_SORT_ONESWEEP=1 selects the
   // one-sweep passes for 32-bit keys (digit histograms in pack + decoupled look-back in the scatter: 10 instead of 14 words of
-  // traffic per key).  Measured on B200 (c2, 4e8 keys): 3.06 ms per one-sweep pass against 2.19 ms for the three kernels - the
-  // look-back walks ~6 predecessor tiles per digit with dependent L2 round trips while the scatter is issue-bound, not
-  // HBM-bound, so removing a read of the keys buys nothing here (DESIGN.md section 3).  Kept, tested, not the default.
+  // traffic per key).  The look-back walks several predecessor tiles per digit with dependent L2 round trips while the
+  // scatter is issue-bound, not HBM-bound, so removing a read of the keys need not pay.  Kept, tested, not the default.
   const char* os_env = getenv("ANV_SORT_ONESWEEP");
   const bool legacy = !(os_env && os_env[0] == '1') || sizeof(K) != 4;
   ANV_CUDA(cudaMemsetAsync(P.state, 0, (size_t)n_cols * sizeof(ColState), st));

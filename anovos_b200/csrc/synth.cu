@@ -193,7 +193,7 @@ extern "C" int anv_synth_f32_rows(float* data, uint32_t* validity, int64_t n_row
   }
   if (n_rows == 0) return ANV_OK;
   const int64_t n4 = (n_rows + 3) / 4;
-  const int blocks = (int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   anv::synth_f32_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(data, validity, n_rows, row0, anv::make_key(seed, column), family,
                                                                   a, b, null_rate);
   ANV_CUDA(cudaGetLastError());
@@ -213,7 +213,7 @@ extern "C" int anv_synth_codes_rows(int32_t* data, uint32_t* validity, int64_t n
   }
   if (n_rows == 0) return ANV_OK;
   const int64_t n4 = (n_rows + 3) / 4;
-  const int blocks = (int)((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int blocks = (int)((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   // span = (card+1)^(1-s) - 1 and inv = 1/(1-s) in double on the host (the NumPy twin does the same), rounded to float once
   const double oms = 1.0 - (double)zipf_s;
   const float span = (float)(pow((double)cardinality + 1.0, oms) - 1.0);

@@ -108,7 +108,7 @@ def _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_conf
         raise TypeError("Invalid input for Column(s)")
     binned = bool(num) and bool(encoding_configs)
     if binned and encoding_configs.get("monotonicity_check", 0) == 1:
-        raise NotImplementedError("monotonic_binning is outside the B200 hot-path build")
+        raise NotImplementedError("monotonic_binning is outside the GPU hot-path build")
     return fr, cols, num, cat, ev_w, nev_w, binned
 
 

@@ -105,7 +105,7 @@ def nullColumns_detection(spark, idf, list_of_cols="missing", drop_cols=[], trea
                 print("Before Count: " + str(fr.count()))
                 print("After Count: " + str(odf.count()))
         else:
-            raise NotImplementedError("treatment_method=%r (imputation) is outside the B200 hot-path build" % treatment_method)
+            raise NotImplementedError("treatment_method=%r (imputation) is outside the GPU hot-path build" % treatment_method)
     out = ResultFrame(stats)
     if print_impact:
         out.show(len(cols))

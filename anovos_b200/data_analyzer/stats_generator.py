@@ -1,4 +1,4 @@
-"""B200 implementation of `anovos.data_analyzer.stats_generator` (reference
+"""CUDA implementation of `anovos.data_analyzer.stats_generator` (reference
 /root/reference/src/main/anovos/data_analyzer/stats_generator.py:33-1011): same function
 names, arguments, output columns, rounding and error behaviour; `spark` is accepted and
 ignored (it may be None), `idf` is anything `anovos_b200.frame.as_frame` accepts.  All

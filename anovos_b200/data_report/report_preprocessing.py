@@ -14,7 +14,7 @@ def save_stats(spark, idf, master_path, function_name, reread=False, run_type="l
     `<master_path>/<function_name>.csv` with a header row and no index, exactly what `idf.toPandas().to_csv(...,
     index=False)` gives in the reference (:92).  reread=True returns the file read back with inferSchema (:121-127)."""
     if run_type != "local":
-        raise NotImplementedError("save_stats: run_type %r (cloud copies are outside the B200 hot-path build)" % run_type)
+        raise NotImplementedError("save_stats: run_type %r (cloud copies are outside the GPU hot-path build)" % run_type)
     local_path = master_path
     if mlflow_config is not None and mlflow_config.get("track_reports", False):
         local_path = local_path + "/" + mlflow_config["run_id"]

@@ -1,4 +1,4 @@
-"""B200 implementation of `anovos.data_transformer.transformers.attribute_binning`
+"""CUDA implementation of `anovos.data_transformer.transformers.attribute_binning`
 (reference /root/reference/src/main/anovos/data_transformer/transformers.py:87-291).
 
 The reference computes the cutoffs with one Spark agg (equal_range, :216-232) or

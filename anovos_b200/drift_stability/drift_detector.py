@@ -1,4 +1,4 @@
-"""B200 implementation of `anovos.drift_stability.drift_detector.statistics` (reference
+"""CUDA implementation of `anovos.drift_stability.drift_detector.statistics` (reference
 /root/reference/src/main/anovos/drift_stability/drift_detector.py:16-371).
 
 Data path: source frame -> K1 (min/max) -> cutoffs on the host (bit-identical model) ->

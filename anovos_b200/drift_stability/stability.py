@@ -1,4 +1,4 @@
-"""B200 implementation of `anovos.drift_stability.stability.stability_index_computation`
+"""CUDA implementation of `anovos.drift_stability.stability.stability_index_computation`
 (reference /root/reference/src/main/anovos/drift_stability/stability.py:15-332): the inner
 loop of the reference - one `select(mean, stddev, kurtosis)` Spark job per column per dataset
 (:239-245) - is exactly the fused moments kernel (K1), one launch per dataset; the rest is a

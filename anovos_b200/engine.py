@@ -400,7 +400,7 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
     then returns (list, float64 [n_cols, n_ranks]) with the exact order statistics.
     Default: the batched LSD radix sort (anv_mode_distinct).  sort_algorithm = "partition" sends 32-bit columns through
     the partition + count path (anv_mode_distinct_partition: no sort, ~3 words of traffic per key, but its per-key global
-    atomics make it slower than the sort on B200 - DESIGN.md section 3); a column that path hands back (mode_rows == -2)
+    atomics can make it slower than the sort - DESIGN.md section 3); a column that path hands back (mode_rows == -2)
     is redone by the sort.  All column batches of a call are enqueued back to back on the stream into one workspace (stream
     order makes the reuse safe) and the results come back in ONE device-to-host copy."""
     if getattr(frame, "is_partitioned", False):

@@ -1,4 +1,4 @@
-"""Columnar frame: the `idf` of the B200 path.
+"""Columnar frame: the `idf` of the GPU path.
 
 The reference passes Spark DataFrames (`idf`) into every function of the hot path;
 here `idf` is a ColumnFrame: column-major device buffers (one contiguous torch CUDA

@@ -1,4 +1,4 @@
-"""Result object of the B200 path: the small per-attribute frames the reference returns as
+"""Result object of the GPU path: the small per-attribute frames the reference returns as
 Spark DataFrames.  Callers of the reference immediately do `.toPandas().to_csv(...)`
 (data_report/report_preprocessing.py:92), `.show(n)` (workflow.py:509), `.count()` or
 `.where(F.col("attribute") == x)` (reference tests); this class offers that surface on top

@@ -2,10 +2,11 @@
 """bench.py - the measurement contract of this repo.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c3|c2|c3f32|c4|c5|c1] [--impl ours|reference]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic input: the FULL stats_generator
 (measures_of_counts / centralTendency / cardinality / dispersion / percentiles / shape) of a synthetic frame that is
-already resident in HBM.  Default workload = BASELINE.json configs[2], the north-star configuration: 100 M rows x 200
+already resident in HBM.  Default workload = BASELINE.json configs[2], the north-star configuration: 40 M rows x 200
 mixed columns (150 float32 + 50 dictionary-coded string columns; `c3f32` is the all-float32 variant, `c2` =
 configs[1], 10 M x 50).  Rank 0 prints ONE JSON line.  `value` = rows x cols / s over all ranks (weak scaling: every
 rank owns `cols` columns - columns shard with no data-path collective, one NCCL all_gather of the per-column summaries
@@ -14,7 +15,9 @@ process bound to the GPU's NUMA node).  `roofline` describes the dominant C call
 other calls, all timed with CUDA events inside the timed region; `fused_stats_hist_pass` = the north-star kernel (moments
 + histogram in one read) and drift statistics on the same frame; `parity` = the step's own results checked against the
 oracle on the bit-identical NumPy twin of the generator (outside the timed region).  `--impl reference` times the CPU
-oracle restatement on the host cores (Spark is not available on the box).
+oracle restatement on the host cores (Spark is not available on the box).  `--dump-outputs DIR` writes what the last timed
+step returned (the numeric cells of its result tables) as DIR/<function>.<column>.npy in float64; the inputs are seeded, so
+two builds can be compared output for output.
 """
 import argparse
 import json
@@ -29,11 +32,12 @@ if ROOT not in sys.path:
 
 WORKLOADS = {
     "c2": dict(rows=10_000_000, cols=50, cat_every=0, desc="synthetic 10M rows x 50 float32 cols: full stats_generator"),
-    # BASELINE.json configs[2] / north_star target: 75 % numeric / 25 % categorical (SURVEY.md 8d)
-    "c3": dict(rows=100_000_000, cols=200, cat_every=4,
-               desc="synthetic 100M rows x 200 mixed num/cat cols (150 float32 + 50 dictionary-coded string): "
+    # BASELINE.json configs[2] / north_star target: 75 % numeric / 25 % categorical (SURVEY.md 8d).  40 M rows keep the frame
+    # (32 GB) resident next to the sort scratch (engine.SORT_WORKSPACE_BUDGET) and a drift target in the 80 GB of an H100.
+    "c3": dict(rows=40_000_000, cols=200, cat_every=4,
+               desc="synthetic 40M rows x 200 mixed num/cat cols (150 float32 + 50 dictionary-coded string): "
                     "stats_generator + histogram binning"),
-    "c3f32": dict(rows=100_000_000, cols=200, cat_every=0, desc="synthetic 100M rows x 200 float32 cols: full stats_generator"),
+    "c3f32": dict(rows=40_000_000, cols=200, cat_every=0, desc="synthetic 40M rows x 200 float32 cols: full stats_generator"),
     "tiny": dict(rows=200_000, cols=8, cat_every=4, desc="smoke-size synthetic frame"),
     # BASELINE.json configs[0], the reference's own CPU-runnable plumbing check (SURVEY.md 8d: "always report C1")
     "c1": dict(rows=32_561, cols=17, c1=True, desc="income dataset (data/test_dataset, 32 561 x 17: 7 int + 1 double + 9 string): "
@@ -68,7 +72,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 def settle_gc():
@@ -167,15 +171,35 @@ class ClockSampler:
 # the step
 # ---------------------------------------------------------------------------------------------
 
+STATS_FUNCTIONS = ["measures_of_counts", "measures_of_centralTendency", "measures_of_cardinality", "measures_of_dispersion",
+                   "measures_of_percentiles", "measures_of_shape"]
+
+
+def dump_outputs(path, names, frames):
+    """--dump-outputs: the numeric cells of every column of each result table as <path>/<name>.<column>.npy (float64, finite).
+    Where a column also holds null or non-numeric cells (the mean of a string column is null, its mode a string), only the
+    numeric cells are written and <path>/<name>.<column>.rows.npy holds their row numbers in the table, so two dumps still
+    line up value for value."""
+    import numpy as np
+    import pandas as pd
+    os.makedirs(path, exist_ok=True)
+    for name, df in zip(names, frames):
+        for col in df.columns:
+            v = pd.to_numeric(df[col], errors="coerce").to_numpy(dtype=np.float64, na_value=np.nan)
+            keep = np.isfinite(v)
+            if not keep.any():
+                continue       # a column of labels (`attribute`, `flagged` strings) or of nulls only: nothing numeric to compare
+            np.save(os.path.join(path, "%s.%s.npy" % (name, col)), v[keep])
+            if not keep.all():
+                np.save(os.path.join(path, "%s.%s.rows.npy" % (name, col)), np.flatnonzero(keep).astype(np.float64))
+
+
 def stats_step(frame, keep_cache=False):
     """Full stats_generator through the public API; returns the result frames (pandas)."""
     import anovos.data_analyzer.stats_generator as sg
     if not keep_cache:
         frame._cache = {k: v for k, v in frame._cache.items() if isinstance(k, tuple) and k and k[0] == "desc"}
-    out = [sg.measures_of_counts(None, frame), sg.measures_of_centralTendency(None, frame),
-           sg.measures_of_cardinality(None, frame), sg.measures_of_dispersion(None, frame),
-           sg.measures_of_percentiles(None, frame), sg.measures_of_shape(None, frame)]
-    return [o.toPandas() for o in out]
+    return [getattr(sg, fn)(None, frame).toPandas() for fn in STATS_FUNCTIONS]
 
 
 class StdoutGuard:
@@ -209,7 +233,7 @@ KERNEL_NAMES = {
     "anv_hist": "scan_kernel<HIST> (anv_hist: binning + histogram)",
     "anv_moments_hist": "scan_kernel<MOM+HIST> (anv_moments_hist: moments + histogram in one read)",
 }
-# what limits each call (ncu evidence under profiles/): the roofline fraction is always quoted against HBM
+# what is expected to limit each call (by design: the sort and HLL++ are instruction-bound); the roofline fraction is always quoted against HBM
 BOUND = {"anv_mode_distinct": "issue", "anv_mode_distinct_partition": "l2 (per-key atomics and 4-byte stores)", "anv_hll_registers": "issue",
          "anv_moments_hist": "issue"}
 
@@ -293,6 +317,8 @@ def _run_ours(args, out):
     launches = engine.launch_count - l0
     kt = engine.timer.totals()
     engine.timer = None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, STATS_FUNCTIONS, last)
     t = torch.tensor([ms], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -306,17 +332,6 @@ def _run_ours(args, out):
     num = [c for c in src.columns if src.column(c).kind == "num"]
     n_keys = int(sum(int(v) for v in engine.moments(src, num)["n_nonzero"])) if num else 0   # exact zeros are counted, not sorted
     peak, peak_src = peaks()
-    traffic_tbl, traffic_src = {}, None
-    for cand in sorted(os.listdir(os.path.join(ROOT, "profiles")), reverse=True):   # newest round first
-        if not (cand.startswith("r") and "traffic" in cand and cand.endswith(".json")):
-            continue
-        try:  # dram__bytes_read+write per call from a committed ncu capture of the SAME workload
-            tj = json.load(open(os.path.join(ROOT, "profiles", cand)))
-            if tj.get("rows") == rows and tj.get("cols") == cols and tj.get("cat_every", 0) == cat_every:
-                traffic_tbl, traffic_src = tj["dram_bytes_per_launch"], "profiles/" + cand
-                break
-        except Exception:
-            pass
 
     def roof(call):
         v = kt[call]
@@ -328,26 +343,23 @@ def _run_ours(args, out):
         elif call == "anv_mode_distinct_partition":
             alg += n_keys * 4 * PARTITION_WORDS_PER_KEY
         ach = alg / (ms_step * 1e-3) / 1e9 if (alg and ms_step > 0) else None
-        traffic = traffic_tbl.get(call)
         more = {}
         if call == "anv_mode_distinct" and ms_step > 0:
-            # context for an issue-bound kernel: keys sorted per second (pack, run summaries and HLL++ registers included in the
-            # time) next to the CUDA toolkit's radix sort on the same GPU (recorded by scripts/yardstick/cub_sort.cu)
-            more = {"sorted_keys_per_step": n_keys, "gkeys_per_s_incl_pack_and_summaries": n_keys / (ms_step * 1e-3) / 1e9,
-                    "library_yardstick": library_yardstick(rows)}
+            # context for an issue-bound kernel: keys sorted per second (pack, run summaries and HLL++ registers included in the time)
+            more = {"sorted_keys_per_step": n_keys, "gkeys_per_s_incl_pack_and_summaries": n_keys / (ms_step * 1e-3) / 1e9}
         return {**more, "kernel": KERNEL_NAMES.get(call, {"anv_mode_distinct": SORT_DESIGN, "anv_mode_distinct_partition": PARTITION_DESIGN}.get(call, call)),
                 "call": call,
                 "bound": BOUND.get(call, "hbm"), "achieved": ach, "peak": peak,
                 "peak_source": peak_src, "unit": "GB/s", "frac": ach / peak if ach else None,
-                "traffic": traffic if traffic else None, "traffic_source": traffic_src if traffic else None,
+                "traffic": None,
                 "algorithmic_bytes_per_launch": alg / per_step if alg else None,
                 "ms_per_launch": ms_step / per_step, "launches_per_step": per_step,
                 "share_of_step": v["ms"] / ms if ms > 0 else None}
     by_share = sorted(kt, key=lambda c: -kt[c]["ms"])
     roofline = roof(by_share[0]) if by_share else None
     if roofline is not None and roofline["bound"] != "hbm":
-        roofline["note"] = ("bound by instruction issue, not by HBM (ncu: profiles/); frac is still achieved algorithmic GB/s over the "
-                            "measured HBM peak - see roofline_kernels for the HBM-bound scan kernels the step also runs")
+        roofline["note"] = ("bound by instruction issue, not by HBM; frac is still achieved algorithmic GB/s over the "
+                            "HBM peak - see roofline_kernels for the HBM-bound scan kernels the step also runs")
     roofline_kernels = [roof(c) for c in by_share[1:]]
     kernels = {k: {"ms_per_step": v["ms"] / args.steps, "calls_per_step": v["calls"] / args.steps,
                    "share_of_step": v["ms"] / ms} for k, v in sorted(kt.items())}
@@ -395,7 +407,7 @@ def _run_ours(args, out):
                 parity = {"skipped": "N > 1 runs the identical per-rank path on other column ids: see the N = 1 line (or pass --parity)"}
             # ---- e2e: same step from pinned HOST buffers through the public API ---------------------
             holder = [src]
-            src = None   # the leg frees the resident frame once it is copied: at c3 (80 GB) it would not fit twice
+            src = None   # the leg frees the resident frame once it is copied: it need not fit twice
             try:
                 e2e = e2e_numbers(args, rows, cols, holder, torch, framemod, engine, dist=dist if e2e_all else None, world=world)
                 e2e["numa"] = numa
@@ -422,20 +434,6 @@ def _run_ours(args, out):
         dist.destroy_process_group()
     if line is not None:
         out.emit(json.dumps(line))
-
-
-def library_yardstick(rows):
-    """cub::DeviceRadixSort::SortKeys (bare sort of uniform 32-bit keys) as recorded under profiles/ for this row count."""
-    for cand in sorted(os.listdir(os.path.join(ROOT, "profiles")), reverse=True):
-        if "cub_yardstick" in cand and cand.endswith(".json"):
-            try:
-                for e in json.load(open(os.path.join(ROOT, "profiles", cand)))["library"]:
-                    if e["key_bits"] == 32 and e["n_keys"] == rows:
-                        return {"library": e["library"], "gkeys_per_s": e["gkeys_per_s"], "ms_per_column": e["ms_per_column"],
-                                "what": "bare key sort, no pack / run summaries / HLL++", "source": "profiles/" + cand}
-            except Exception:
-                pass
-    return None
 
 
 def rowslab_check(rank, world, torch, dist):
@@ -522,8 +520,7 @@ def parity_check(rows, cols, first_col, cat_every, src, frames, drift_res):
     exp = cpu_bench.oracle_columns(lambda c, seed, shifted: synth.host_table(rows, 1, seed=seed, shifted=shifted, columns=[c],
                                                                            cat_every=cat_every), ids, drift_ids)
     names = ["c%04d" % c for c in ids]
-    fn_names = ["measures_of_counts", "measures_of_centralTendency", "measures_of_cardinality", "measures_of_dispersion",
-                "measures_of_percentiles", "measures_of_shape"]
+    fn_names = STATS_FUNCTIONS
     cells = bad = 0
     worst, examples = 0.0, []
     for fn, got in zip(fn_names, frames):
@@ -632,6 +629,8 @@ def _run_c1(args, out, wl, world, rank, local):
     kt = engine.timer.totals()
     engine.timer = None
     launches = engine.launch_count - l0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ["measures_of_centralTendency"], [res])
     h0, d0 = framemod.h2d_bytes, engine.d2h_bytes
     t0 = time.perf_counter()
     for _ in range(args.steps):
@@ -754,6 +753,9 @@ def _run_stream(args, out, wl, rows, cols, world, rank, local):
     launches = engine.launch_count - l0
     kt = engine.timer.totals()
     engine.timer = None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ["statistics", "source.measures_of_counts", "source.measures_of_shape",
+                                         "target.measures_of_counts", "target.measures_of_shape"], res)
     gen_ms = generation_only()
     t = torch.tensor([ms, gen_ms], dtype=torch.float64, device="cuda")
     if world > 1:
@@ -877,16 +879,17 @@ def fused_pass_numbers(src, rows, names, peak, torch, engine):
         out[name] = {"ms_per_launch": ms, "algorithmic_bytes_per_launch": alg_bytes, "achieved_gbs": gbs, "frac_of_peak": gbs / peak,
                      "rows_cols_per_s": rows * len(names) / (ms * 1e-3)}
     out["fused"]["loop"] = ("8 x 128-bit loads per thread in registers (default); ANV_FUSED_STAGED=1: null-free columns through a "
-                            "thread-private cp.async ring instead (A/B: profiles/r2b_fused_ab.md)")
+                            "thread-private cp.async ring instead")
     return out
 
 
 def drift_numbers(args, src, rows, cols, rank, cat_every, torch, engine, synth):
     """drift_detector.statistics(target, source, method_type="all", use_sampling=False) through the public
     API on two device-resident frames: source K1 + K2, target fused K1+K2 in one read, K3 reduce.  When source + target
-    do not fit HBM together (c3: 2 x 80 GB) the call covers the first columns whose target still fits."""
+    do not fit HBM together the call covers the first columns whose target still fits."""
     import tempfile
     import anovos.drift_stability.drift_detector as dd
+    torch.cuda.empty_cache()     # the step's cached sort scratch is free for the target frame
     free = torch.cuda.mem_get_info()[0]
     n = int(min(cols, max(0, (free - (24 << 30)) // (rows * 4 + rows // 8 + 1))))
     if n < 1:
@@ -1151,6 +1154,8 @@ def main():
     ap.add_argument("--cols", type=int, default=0)
     ap.add_argument("--chunk", type=int, default=0, help="rows per chunk of the streamed workloads (c4, c5)")
     ap.add_argument("--no-extras", action="store_true", help="profiling runs: skip e2e / cpu_baseline / fused extras")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the result tables of the last timed step as DIR/<function>.<column>.npy (float64)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

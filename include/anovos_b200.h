@@ -1,5 +1,5 @@
 /*
- * anovos_b200.h - C ABI of libanovos_b200.so: the B200 (sm_100a) kernels behind the
+ * anovos_b200.h - C ABI of libanovos_b200.so: the H100 (sm_90a) kernels behind the
  * Anovos stats_generator / attribute_binning / drift_detector hot path.
  *
  * The reference (anovos/anovos v1.1.0) has NO native / FFI interface: its boundary is the

@@ -60,7 +60,7 @@ def run(flag):
 
 def sustained(flag, launches=80):
     """Enqueue `launches` back to back and sample NVML (SM clock, power, throttle reasons) while they run: the pass is
-    FP64- and HBM-heavy, and a B200 under its power cap lowers the SM clock within a few hundred milliseconds."""
+    FP64- and HBM-heavy, and a GPU under its power cap lowers the SM clock within a few hundred milliseconds."""
     import time
     import pynvml
     pynvml.nvmlInit()

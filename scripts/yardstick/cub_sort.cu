@@ -1,6 +1,6 @@
 // Library yardstick for the sort numbers in DESIGN.md §4: cub::DeviceRadixSort::SortKeys (CCCL shipped with CUDA 12.9, the
 // one-sweep implementation) on the same key counts and widths the product's LSD passes handle.  Measurement aid only: the
-// product does not link or call it.  Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o cub_sort cub_sort.cu
+// product does not link or call it.  Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o cub_sort cub_sort.cu
 // Usage: cub_sort <n_keys> <n_columns> <bits: 32|64> [reps]  -> one JSON line (keys/s over all columns, ms per column).
 #include <cub/device/device_radix_sort.cuh>
 #include <cstdio>
@@ -20,7 +20,7 @@ __global__ void fill(uint32_t* p, size_t n_words, uint32_t seed) {
 template <typename K> static int run(size_t n, int cols, int reps) {
   K *in, *out; void* tmp = nullptr; size_t tmp_bytes = 0;
   if (cudaMalloc(&in, n * sizeof(K) * cols) != cudaSuccess || cudaMalloc(&out, n * sizeof(K)) != cudaSuccess) { fprintf(stderr, "alloc failed\n"); return 1; }
-  fill<<<148 * 8, 256>>>((uint32_t*)in, n * cols * (sizeof(K) / 4), 7u);
+  fill<<<132 * 8, 256>>>((uint32_t*)in, n * cols * (sizeof(K) / 4), 7u);
   cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, in, out, n);
   cudaMalloc(&tmp, tmp_bytes);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);

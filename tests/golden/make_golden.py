@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Generate the golden fixtures under tests/golden/ from the reference checkout.
+"""Generate the golden fixtures under tests/golden/ from a checkout of anovos/anovos.
 
-Run in the build container only (needs /root/reference, which does not exist on
-the GPU box); the outputs are committed.  Nothing here executes reference code
+    python tests/golden/make_golden.py <path of the anovos checkout>
+
+The outputs are committed, so the tests never need the checkout.  Nothing here executes reference code
 (it needs a JVM + Spark, absent here): the vectors are the REAL Spark outputs the
 reference stores in its notebooks, plus the input datasets they were computed on.
 
@@ -23,12 +24,13 @@ import html.parser
 import json
 import os
 import shutil
+import sys
 
 import pyarrow as pa
 import pyarrow.csv as pacsv
 import pyarrow.parquet as pq
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "."
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 INT_COLS = ["age", "fnlwgt", "education-num", "capital-gain", "capital-loss", "hours-per-week", "dupl_age"]
