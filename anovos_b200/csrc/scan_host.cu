@@ -34,8 +34,12 @@ __global__ void __launch_bounds__(32) finalize_moments(const Partial* partials, 
   if (lane == 0) {
     anv_moments_t r;
     r.n_valid = n; r.n_nonzero = nz;
-    if (n > 0) { r.min = mn; r.max = mx; r.mean = acc.mean; r.m2 = acc.m2; r.m3 = acc.m3; r.m4 = acc.m4; }
-    else { r.min = r.max = r.mean = nan(""); r.m2 = r.m3 = r.m4 = 0.0; }
+    if (n > 0) {
+      r.mean = acc.mean; r.m2 = acc.m2; r.m3 = acc.m3; r.m4 = acc.m4;
+      // min / max skip NaN; with nothing but NaN they are NaN (as the order statistics are), not the start values
+      if (mn > mx) mn = mx = nan("");
+      r.min = mn; r.max = mx;
+    } else { r.min = r.max = r.mean = nan(""); r.m2 = r.m3 = r.m4 = 0.0; }
     out[c] = r;
   }
 }

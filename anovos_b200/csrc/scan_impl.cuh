@@ -216,6 +216,17 @@ struct ScanShared {  // declared once in the kernel (not per template instantiat
   int fix;
 };
 
+// Tile power sums t_k = sum (x - pivot)^k over n valid rows -> central form (mean, M2, M3, M4).  The cancellation is
+// bounded by the tile's spread around the pivot, so the pivot must be an element of the tile.
+__device__ __forceinline__ void central_from_power_sums(Partial& out, double pivot, double t1, double t2, double t3,
+                                                        double t4) {
+  const double dl = t1 / (double)out.n;  // mean - pivot
+  out.mean = pivot + dl;
+  out.m2 = t2 - t1 * dl;
+  out.m3 = t3 - 3.0 * dl * t2 + 2.0 * dl * dl * t1;
+  out.m4 = t4 - 4.0 * dl * t3 + 6.0 * dl * dl * t2 - 3.0 * dl * dl * dl * t1;
+}
+
 // ---- the tile body --------------------------------------------------------------------
 // HPATH: -1 no histogram, 0 private per-thread counters, 1 per-CTA shared atomics, 2 global atomics
 template <typename T, bool MOM, int HPATH, bool ASSIGN, bool NULLS, int MODE, bool STAGED = false>
@@ -605,12 +616,7 @@ __device__ __forceinline__ void scan_tile(const ScanParams& P, const anv_column_
       out.n = n; out.nz = nz; out.mn = a; out.mx = b;
       if (n > 0) {
         // the power sums ran over n_tile lanes (null lanes contributed d == 0): shift to the mean of the n valid ones
-        const double dn = (double)n;
-        const double dl = t1 / dn;  // mean - pivot
-        out.mean = pivot + dl;
-        out.m2 = t2 - t1 * dl;
-        out.m3 = t3 - 3.0 * dl * t2 + 2.0 * dl * dl * t1;
-        out.m4 = t4 - 4.0 * dl * t3 + 6.0 * dl * dl * t2 - 3.0 * dl * dl * dl * t1;
+        central_from_power_sums(out, pivot, t1, t2, t3, t4);
       } else {
         out.mean = 0.0; out.m2 = out.m3 = out.m4 = 0.0;
       }
@@ -618,31 +624,60 @@ __device__ __forceinline__ void scan_tile(const ScanParams& P, const anv_column_
       if (NULLS) SS.fix = (!have_pivot && n > 0) ? 1 : 0;
     }
     if (NULLS) {
-      // Rare repair: no finite non-null value among the first 1024 rows, so null lanes
-      // impersonated 0, which is not an element and may have polluted min / max.
+      // Rare repair: no finite non-null value among the first 1024 rows, so null lanes impersonated 0.  0 is not an
+      // element: it may have polluted min / max, and power sums taken around 0 lose the spread to cancellation when the
+      // values sit far from 0 (a column that starts partway through a table).  Redo the tile around its first finite
+      // valid element.  A tile without one keeps pivot 0: its sums are NaN / inf whatever the pivot.
       __syncthreads();
       if (SS.fix) {
-        double a = INFINITY, b = -INFINITY;
+        int first = n_tile;
+        for (int row = tid; row < n_tile; row += ANV_BLOCK) {
+          if (((vwords[row >> 5] >> (row & 31)) & 1u) && isfinite(Traits<T>::to_double(data[row]))) {
+            first = row;
+            break;
+          }
+        }
+        first = __reduce_min_sync(ANV_FULL, first);
+        if (lane == 0) SS.redn[warp][0] = (uint32_t)first;
+        __syncthreads();
+        for (int w = 0; w < ANV_WARPS; ++w) first = min(first, (int)SS.redn[w][0]);
+        const double pv = first < n_tile ? Traits<T>::to_double(data[first]) : 0.0;
+        double a = INFINITY, b = -INFINITY, u1 = 0.0, u2 = 0.0, u3 = 0.0, u4 = 0.0;
         for (int row = tid; row < n_tile; row += ANV_BLOCK) {
           if ((vwords[row >> 5] >> (row & 31)) & 1u) {
             const double v = Traits<T>::to_double(data[row]);
             a = fmin(a, v);
             b = fmax(b, v);
+            const double d = v - pv, d2 = d * d;
+            u1 += d;
+            u2 += d2;
+            u3 = fma(d2, d, u3);
+            u4 = fma(d2, d2, u4);
           }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
           a = fmin(a, shfl_down_d(a, o));
           b = fmax(b, shfl_down_d(b, o));
+          u1 += shfl_down_d(u1, o);
+          u2 += shfl_down_d(u2, o);
+          u3 += shfl_down_d(u3, o);
+          u4 += shfl_down_d(u4, o);
+        }
+        if (lane == 0) {
+          SS.red[warp][0] = u1; SS.red[warp][1] = u2; SS.red[warp][2] = u3; SS.red[warp][3] = u4;
+          SS.red[warp][4] = a; SS.red[warp][5] = b;
         }
         __syncthreads();
-        if (lane == 0) { SS.red[warp][4] = a; SS.red[warp][5] = b; }
-        __syncthreads();
         if (tid == 0) {
-          for (int w = 1; w < ANV_WARPS; ++w) { a = fmin(a, SS.red[w][4]); b = fmax(b, SS.red[w][5]); }
+          for (int w = 1; w < ANV_WARPS; ++w) {  // fixed order: deterministic
+            u1 += SS.red[w][0]; u2 += SS.red[w][1]; u3 += SS.red[w][2]; u4 += SS.red[w][3];
+            a = fmin(a, SS.red[w][4]); b = fmax(b, SS.red[w][5]);
+          }
           Partial& out = P.partials[(size_t)c * P.tiles_per_col + blockIdx.x];
           out.mn = a;
           out.mx = b;
+          central_from_power_sums(out, pv, u1, u2, u3, u4);
         }
       }
     }

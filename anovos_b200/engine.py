@@ -179,6 +179,13 @@ class BinModel:
                     else np.spacing(max(abs(mn), abs(mx)))
                 ok = (w > 0 and math.isfinite(w) and np.all(np.isfinite(th)) and np.all(np.diff(th) > 0)
                       and w >= 8 * float(ulp) and nb < (1 << 20))
+                # the guess runs in the column's type: x - lo over the range and the scales 1/w and 1/(w (B-1)) must be
+                # finite normal numbers of it (a range wider than FLT_MAX overflows; a subnormal width overflows 1/w)
+                T = np.float32 if col.anv_dtype == _lib.ANV_F32 else np.float64
+                with np.errstate(over="ignore", divide="ignore", invalid="ignore"):
+                    scales = np.array([1.0 / w, 1.0 / (w * max(nb - 1, 1))]).astype(T) if ok else np.zeros(2, T)
+                    ok = ok and bool(np.isfinite(T(mx) - T(mn)) and np.all(np.isfinite(scales))
+                                     and np.all(scales >= np.finfo(T).tiny))
                 if ok:
                     mode, lo, inv_w = 1, mn, 1.0 / w
             specs[i] = (len(cut) + 1, mode, lo, inv_w, off)

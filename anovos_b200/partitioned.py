@@ -39,7 +39,9 @@ from .frame import ColumnFrame
 def merge_moments(parts):
     """Merge per-partition moment records (engine._MOM_DT arrays, one row per column) in the order
     given.  The same algebra as the device-side tile merge (csrc/common.cuh merge_central) and as
-    Spark's CentralMomentAgg.merge; min/max follow Spark's NaN-is-largest ordering."""
+    Spark's CentralMomentAgg.merge; min/max follow Spark's NaN-is-largest ordering, except that a partition of
+    nothing but NaN (min = max = NaN, as finalize_moments reports it) adds no extrema: a frame split into row
+    partitions then has the extrema of the same frame held whole.  Both sides all-NaN give NaN."""
     acc = np.array(parts[0], copy=True)
     for b in parts[1:]:
         a = acc
@@ -58,6 +60,8 @@ def merge_moments(parts):
                   + 6.0 * dn2 * (na * na * b["m2"] + nb * nb * a["m2"]) + 4.0 * dn * (na * b["m3"] - nb * a["m3"]))
             mn = np.fmin(a["min"], b["min"])           # NaN only when both sides are all-NaN
             mx = np.maximum(a["max"], b["max"])        # NaN (largest in Spark's order) propagates
+            a_nan, b_nan = np.isnan(a["min"]) & np.isnan(a["max"]), np.isnan(b["min"]) & np.isnan(b["max"])
+            mx = np.where(a_nan, b["max"], np.where(b_nan, a["max"], mx))   # all-NaN partitions add no extrema
         out = np.array(a, copy=True)
         for f, v in (("mean", mean), ("m2", m2), ("m3", m3), ("m4", m4), ("min", mn), ("max", mx)):
             out[f] = np.where(both, v, np.where(only_b, b[f], a[f]))

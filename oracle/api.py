@@ -890,7 +890,7 @@ def _encoded_groups(table, col, encoding_configs):
         if p.n == 0:
             return np.array([None] * p.N, dtype=object)
         cut = p.equal_frequency_cutoffs(bs) if bm == "equal_frequency" else S.equal_range_cutoffs(*p.minmax(), bs)
-        ids = S.assign_bins(p.values.astype(np.float64), p.valid, cut, bs)
+        ids = S.assign_bins(p.values, p.valid, cut, bs)
         return np.array([int(k) if ok else None for k, ok in zip(ids, p.valid)], dtype=object)
     return np.array([(v if ok else None) for v, ok in zip(p.values.tolist(), p.valid)], dtype=object)
 

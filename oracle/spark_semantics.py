@@ -452,13 +452,32 @@ def equal_frequency_cutoffs(sorted_x64: np.ndarray, bin_size: int):
     return [float(sorted_x64[gk_query_position(sm, n, APPROX_QUANTILE_EPS, j * w)]) for j in range(1, bin_size)]
 
 
-def assign_bins(x64: np.ndarray, valid: np.ndarray, cutoffs, bin_size: int) -> np.ndarray:
+def assign_bins(x: np.ndarray, valid: np.ndarray, cutoffs, bin_size: int) -> np.ndarray:
     """bucket_label (transformers.py:248-271), bin_dtype="numerical":
     null -> 0 here (None in the reference); first i with v <= cut[i] -> i+1; else
-    len(cutoffs)+1.  == 1 + #(cutoffs strictly below v); NaN lands in the last bin."""
-    cut = np.asarray(cutoffs, dtype=np.float64)
-    idx = np.searchsorted(cut, x64, side="left").astype(np.int32) + 1
-    idx[np.isnan(x64)] = len(cut) + 1
+    len(cutoffs)+1.  == 1 + #(cutoffs strictly below v); NaN lands in the last bin.
+    x holds the column's own values: an integer column compares exactly, as Python compares an int with a
+    float (c < v <=> floor(c) < v), where float64(v) would round above 2^53."""
+    x = np.asarray(x)
+    if x.dtype.kind in "iu":
+        info = np.iinfo(np.int64)
+        below, th = 0, []                            # cutoffs below every int64, int64 floors of the others
+        for c in map(float, cutoffs):
+            if c == -math.inf:
+                below += 1
+            elif math.isfinite(c):
+                t = math.floor(c)
+                if t < info.min:
+                    below += 1
+                elif t < info.max:                   # floor(c) >= INT64_MAX is below no int64
+                    th.append(t)
+        th = np.sort(np.array(th, dtype=np.int64))
+        idx = (np.searchsorted(th, x.astype(np.int64), side="left") + 1 + below).astype(np.int32)
+    else:
+        x64 = x.astype(np.float64)
+        cut = np.asarray(cutoffs, dtype=np.float64)
+        idx = np.searchsorted(cut, x64, side="left").astype(np.int32) + 1
+        idx[np.isnan(x64)] = len(cut) + 1
     idx[~valid] = 0
     return idx
 

@@ -55,7 +55,7 @@ def histogram(fr, model):
     h = np.zeros((len(model.names), model.max_bins + 1), np.uint64)
     for i, n in enumerate(model.names):
         vals, valid = _values(fr, n)
-        ids = S.assign_bins(vals.astype(np.float64), valid, model.cutoffs[i], len(model.cutoffs[i]) + 1)
+        ids = S.assign_bins(vals, valid, model.cutoffs[i], len(model.cutoffs[i]) + 1)
         h[i, :len(model.cutoffs[i]) + 2] = np.bincount(ids, minlength=len(model.cutoffs[i]) + 2)
     return h
 
@@ -178,7 +178,7 @@ def bin_assign(fr, model):
     out = np.zeros((max(len(model.names), 1), fr.n_rows), np.int32)
     for i, n in enumerate(model.names):
         vals, valid = _values(fr, n)
-        out[i] = S.assign_bins(vals.astype(np.float64), valid, model.cutoffs[i], len(model.cutoffs[i]) + 1)
+        out[i] = S.assign_bins(vals, valid, model.cutoffs[i], len(model.cutoffs[i]) + 1)
     return torch.from_numpy(out)[:len(model.names)]
 
 

@@ -77,9 +77,7 @@ def test_histogram_bit_exact(bins):
     ids = engine.bin_assign(fr, model).cpu().numpy()
     for i, c in enumerate(names):
         vals, valid = S.column_values(t, c)
-        exp = S.assign_bins(vals.astype(np.float64), valid, cuts[i], bins)
-        if vals.dtype == np.int64:  # python compares int with float exactly; float64(v) rounds above 2^53 (not hit here)
-            pass
+        exp = S.assign_bins(vals, valid, cuts[i], bins)   # integer columns compare exactly
         assert np.array_equal(ids[i], exp), c                              # bit-exact bin ids
         cnt = np.bincount(exp, minlength=bins + 1)
         assert np.array_equal(h[i, :bins + 1], cnt.astype(np.uint64)), c   # bit-exact counts
@@ -102,7 +100,7 @@ def test_histogram_generic_cutoffs_with_duplicates():
     h = engine.histogram(fr, model)
     for i, c in enumerate(names):
         vals, valid = S.column_values(t, c)
-        exp = S.assign_bins(vals.astype(np.float64), valid, cuts[i], 10)
+        exp = S.assign_bins(vals, valid, cuts[i], 10)
         assert np.array_equal(h[i, :11], np.bincount(exp, minlength=11).astype(np.uint64)), c
 
 
@@ -314,7 +312,7 @@ def test_moments_hist_without_early_pivot():
     assert (h == h2).all()
     for i, nme in enumerate(names):
         vals, valid = S.column_values(t, nme)
-        exp = S.assign_bins(vals.astype(np.float64), valid, cuts[i], 10)
+        exp = S.assign_bins(vals, valid, cuts[i], 10)
         assert np.array_equal(h[i, :11], np.bincount(exp, minlength=11).astype(np.uint64)), nme
         assert m2["min"][i] == m["min"][i] and m2["max"][i] == m["max"][i] and m2["n_nonzero"][i] == m["n_nonzero"][i]
 

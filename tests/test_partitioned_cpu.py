@@ -50,6 +50,19 @@ def test_merge_moments_nan_ordering():
     assert m["n_valid"][0] == 2 and m["min"][0] == 1.0 and m["max"][0] == 2.0 and m["mean"][0] == 1.5
 
 
+def test_merge_moments_all_nan_partition_adds_no_extrema():
+    """A partition of nothing but NaN has min = max = NaN (finalize_moments): the merged extrema are those of the
+    other partitions, as over the frame held whole; all partitions all-NaN give NaN."""
+    a, b = _record([1.0, 2.0]), _record([np.nan, np.nan])
+    assert np.isnan(b["min"][0]) and np.isnan(b["max"][0])
+    for parts in ([a, b], [b, a], [b, a, b]):
+        m = partitioned.merge_moments(parts)
+        assert m["min"][0] == 1.0 and m["max"][0] == 2.0
+        assert m["n_valid"][0] == sum(int(p["n_valid"][0]) for p in parts)
+    m = partitioned.merge_moments([b, b])
+    assert np.isnan(m["min"][0]) and np.isnan(m["max"][0])
+
+
 def _free_port():
     s = socket.socket()
     s.bind(("127.0.0.1", 0))
