@@ -28,6 +28,9 @@ namespace anv {
 #ifndef ANV_SCAT_MINB
 #define ANV_SCAT_MINB 2          // resident scatter CTAs per SM the register budget is tuned for
 #endif
+// 3 compiles to 40 registers with 48 bytes of spills in sort_scatter_kernel<uint32> (12 bytes with the ranks held as 16-bit
+// halves).  It gained 0.3 % at the bench shape (H100 80GB HBM3, 400 W, sort call of 40 M x 150 float32: 72.2-72.4 ms against
+// 72.4-72.7 ms) and 1.5 % at 100 M x 12 (40.1-40.2 against 40.7-40.8 ms), so 2 stays: 64 registers, no spills.
 constexpr int SORT_TILE = 4096;  // keys per CTA
 constexpr int SCAT_THREADS = 512;  // the scatter kernel runs 16 warps x 8 rounds of 32 keys
 constexpr int SCAT_WARPS = SCAT_THREADS / 32;
@@ -391,18 +394,38 @@ __global__ void __launch_bounds__(ANV_BLOCK) sort_bases_kernel(const SortParams<
   }
 }
 
-// Lanes of `act` holding the same 8-bit digit.  Per bit: ballot of "my bit is set", keep the lanes whose bit equals mine
-// (m &= my bit ? ballot : ~ballot).  Written in C++: the same sequence as inline-asm blocks of vote.sync keeps ptxas for
-// sm_90a from finishing the scatter kernels.
+// Lanes of `act` holding the same 8-bit digit.
+// Default: per bit, one small NON-volatile asm block (and, setp, vote.ballot.sync, @!p not) gives the lanes whose bit equals
+// mine, and the 8 masks are ANDed in C++.  ptxas turns this into R2P (7 digit bits into predicates at once), VOTE, a
+// predicated NOT and a LOP3 AND: about 3 instructions per bit.  The same ballots written with __ballot_sync and a C++
+// select compile to 6-7 per bit.  ptxas 12.9 for sm_90a does not finish the scatter kernels when all 8 bits sit in one asm
+// block (selp + lop3 0x60), volatile or not, nor when the ANDs are written as asm lop3 next to these blocks.
+// ANV_PEERS_MATCH=1: one MATCH.ANY over the whole warp, masked with `act` afterwards (lanes past the end of a partial tile
+// hold digit 0: they must take part in the call but match no live lane).  Fewer instructions (sort_scatter_kernel<uint32>
+// 1243 SASS against 1650) but slower on an H100 80GB HBM3 at 400 W, whole anv_mode_distinct call with ranks and HLL++,
+// two alternating runs each: 100 M x 12 float32 47.8-48.2 ms against 40.7-40.8 ms with the ballots, 40 M x 150
+// 83.2-84.5 ms against 72.4-72.7 ms (the C++ ballots before: 43.5-43.7 and 78.1-78.2 ms).
+#ifndef ANV_PEERS_MATCH
+#define ANV_PEERS_MATCH 0
+#endif
 __device__ __forceinline__ uint32_t peers8(uint32_t d, uint32_t act) {
+#if ANV_PEERS_MATCH
+  return __match_any_sync(ANV_FULL, d) & act;
+#else
   uint32_t m = act;
 #pragma unroll
   for (int b = 0; b < 8; ++b) {
-    const bool p = (d >> b) & 1u;
-    const uint32_t bal = __ballot_sync(ANV_FULL, p);
-    m &= p ? bal : ~bal;
+    uint32_t same;
+    asm("{\n\t.reg .pred p;\n\t"
+        "and.b32 %0, %1, %2;\n\t"
+        "setp.ne.u32 p, %0, 0;\n\t"
+        "vote.ballot.sync.b32 %0, p, 0xffffffff;\n\t"
+        "@!p not.b32 %0, %0;\n\t}"
+        : "=r"(same) : "r"(d), "r"(1u << b));
+    m &= same;
   }
   return m;
+#endif
 }
 
 
@@ -592,7 +615,10 @@ __device__ __forceinline__ void scatter_tile(const SortParams<K>& P, const ColSt
   const int src = S.src[P.pass];
   const K* __restrict__ in = (src ? P.buf[1] : P.buf[0]) + (size_t)c * P.stride + t0;
   K* __restrict__ out = (src ? P.buf[0] : P.buf[1]) + (size_t)c * P.stride;
-  for (int i = tid; i < SCAT_WARPS * 256 / 2; i += SCAT_THREADS) reinterpret_cast<uint32_t*>(&wcnt[0][0])[i] = 0;
+  static_assert(SCAT_WARPS * 256 / 2 % SCAT_THREADS == 0, "the counters clear in whole rounds");
+#pragma unroll
+  for (int j = 0; j < SCAT_WARPS * 256 / 2 / SCAT_THREADS; ++j)   // fixed trip count: 4 stores, no loop control
+    reinterpret_cast<uint32_t*>(&wcnt[0][0])[tid + j * SCAT_THREADS] = 0;
   if (!LOOKBACK && tid < 256) gbase[tid] = P.tile_hist[((size_t)c * 256 + tid) * P.n_tiles + tile];
   constexpr int WR = SORT_TILE / SCAT_WARPS / 32;  // 8 rounds per warp
   K key[WR];

@@ -1,15 +1,83 @@
-"""Profile only the sort-based mode/distinct path (ncu --profile-from-start off)."""
+"""Kernel breakdown of one sort_mode_distinct call (the LSD radix sort behind exact mode, distinct count, percentiles and
+HLL++ registers) at the default bench shape: the numeric columns of synth.device_frame(rows, cols, cat_every=4), with the
+summary ranks and hll_p the stats_generator step passes, so the column batching matches the step.
+torch.profiler with CUDA activities; prints ms per call for each kernel family, the card and its power limit, one JSON line.
+Usage: python scripts/prof_sort.py [rows] [cols] [calls] [tag]"""
+import collections
+import json
+import os
+import subprocess
 import sys
+import tempfile
+
+import numpy as np
 import torch
+from torch.profiler import ProfilerActivity, profile
+
 sys.path.insert(0, ".")
 from anovos_b200 import engine, synth
-rows = int(float(sys.argv[1])) if len(sys.argv) > 1 else 10_000_000
-cols = int(sys.argv[2]) if len(sys.argv) > 2 else 8
-fr = synth.device_frame(rows, cols)
-engine.sort_mode_distinct(fr, fr.columns)
+from anovos_b200 import profile as anv_profile
+
+rows = int(float(sys.argv[1])) if len(sys.argv) > 1 else 40_000_000
+cols = int(sys.argv[2]) if len(sys.argv) > 2 else 200
+calls = int(sys.argv[3]) if len(sys.argv) > 3 else 2
+tag = sys.argv[4] if len(sys.argv) > 4 else "default"
+
+FAMILIES = ["pack_kernel", "sort_bases_kernel", "sort_hist_kernel", "sort_totals_kernel", "sort_scan_kernel",
+            "sort_scatter_kernel", "sort_onesweep_kernel", "run_tile_kernel", "run_merge_kernel"]
+
+
+def family(name):
+    for f in FAMILIES:
+        if f in name:
+            return f.replace("_kernel", "").replace("sort_", "")
+    return "other"
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().split("\n")[0]
+        name, plim = [s.strip() for s in q.split(",")]
+        return name, plim
+    except Exception:
+        return torch.cuda.get_device_name(), "unknown"
+
+
+fr = synth.device_frame(rows, cols, cat_every=4)
+num = [n for n in fr.columns if fr.column(n).kind == "num"]
+mom = engine.moments(fr, num)
+ranks = np.array([engine.quantile_ranks(int(mom["n_valid"][i]), anv_profile.SUMMARY_PROBS, anv_profile.SUMMARY_EPS)
+                  for i in range(len(num))], dtype=np.int64)
+
+
+def run():
+    return engine.sort_mode_distinct(fr, num, ranks, hll_p=anv_profile.DEFAULT_HLL_P)
+
+
+run()                                   # warm-up: module load, workspace
 torch.cuda.synchronize()
-torch.cuda.profiler.start()
-engine.sort_mode_distinct(fr, fr.columns)
-torch.cuda.synchronize()
-torch.cuda.profiler.stop()
-print("done")
+with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    for _ in range(calls):
+        run()
+    torch.cuda.synchronize()
+
+with tempfile.TemporaryDirectory() as d:   # the kernel records of the chrome trace: name + duration in us
+    prof.export_chrome_trace(os.path.join(d, "trace.json"))
+    with open(os.path.join(d, "trace.json")) as f:
+        trace = json.load(f)
+ms = collections.Counter()
+launches = collections.Counter()
+for ev in trace["traceEvents"]:
+    if ev.get("cat") == "kernel":
+        f = family(ev["name"])
+        ms[f] += ev["dur"] / 1e3 / calls
+        launches[f] += 1
+total = sum(ms.values())
+gpu, plim = card()
+print("%s, power limit %s; %d rows x %d numeric columns, per call:" % (gpu, plim, rows, len(num)))
+for f, t in sorted(ms.items(), key=lambda kv: -kv[1]):
+    print("  %-10s %8.2f ms  %5.1f %%  (%d launches per call)" % (f, t, 100 * t / total, launches[f] // calls))
+print("  %-10s %8.2f ms" % ("total", total))
+print(json.dumps({"tag": tag, "gpu": gpu, "power_limit": plim, "rows": rows, "numeric_cols": len(num), "calls": calls,
+                  "kernel_ms_per_call": round(total, 3), "ms_per_call": {f: round(t, 3) for f, t in ms.items()}}))
