@@ -22,6 +22,7 @@
 
 #include "common.cuh"
 #include "hll_hash.cuh"
+#include "keysort.cuh"
 
 namespace anv {
 
@@ -1104,6 +1105,70 @@ static int run_mode_distinct(const anv_column_t* cols, int n_cols, int64_t n_row
   }
   run_merge_kernel<K><<<n_cols, 32 * MERGE_WARPS, 0, st>>>(P, mode_value, mode_rows, n_distinct, ranks, n_ranks, rank_values);
   ANV_CUDA(cudaGetLastError());
+  return ANV_OK;
+}
+
+// ---- one caller-filled column of 64-bit keys (keysort.cuh) ----------------------------------------------------------
+// The same three kernels per pass as anv_mode_distinct's default path, on a single column whose keys the caller wrote
+// into buf[0]: no pack kernel (nothing is dropped, zero keys are sorted like any other) and only the passes asked for.
+struct KeySortLayout {
+  size_t state, buf0, buf1, tile_hist, totals, total;
+  explicit KeySortLayout(int64_t n_rows) {
+    const int64_t n_tiles = (n_rows + SORT_TILE - 1) / SORT_TILE;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { size_t at = o; o = (o + bytes + 255) & ~(size_t)255; return at; };
+    state = take(sizeof(ColState));
+    buf0 = take((size_t)(n_rows > 0 ? n_rows : 1) * sizeof(uint64_t));
+    buf1 = take((size_t)(n_rows > 0 ? n_rows : 1) * sizeof(uint64_t));
+    tile_hist = take((size_t)256 * (n_tiles > 0 ? n_tiles : 1) * 4);
+    totals = take((size_t)256 * 4);
+    total = o;
+  }
+};
+
+__global__ void key_sort_init_kernel(ColState* S, int64_t n_rows) {
+  ColState z{};
+  z.n_valid = (unsigned long long)n_rows;
+  *S = z;
+}
+
+size_t key_sort64_workspace_bytes(int64_t n_rows) { return KeySortLayout(n_rows).total; }
+
+void key_sort64_bind(void* workspace, int64_t n_rows, KeySort64* out) {
+  const KeySortLayout L(n_rows);
+  char* w = reinterpret_cast<char*>(workspace);
+  out->buf[0] = reinterpret_cast<uint64_t*>(w + L.buf0);
+  out->buf[1] = reinterpret_cast<uint64_t*>(w + L.buf1);
+  out->cur = &reinterpret_cast<ColState*>(w + L.state)->cur;
+}
+
+int key_sort64(void* workspace, size_t workspace_bytes, int64_t n_rows, int first_pass, int end_pass, cudaStream_t st) {
+  const KeySortLayout L(n_rows);
+  if (workspace_bytes < L.total) { set_error("key_sort64: workspace too small (%zu < %zu)", workspace_bytes, L.total); return ANV_ERR_WORKSPACE; }
+  if (first_pass < 0 || end_pass > 8) { set_error("key_sort64: passes %d..%d outside 0..8", first_pass, end_pass); return ANV_ERR_INVALID; }
+  char* w = reinterpret_cast<char*>(workspace);
+  SortParams<uint64_t> P{};
+  P.n_cols = 1;
+  P.n_rows = n_rows;
+  P.stride = n_rows;
+  P.n_tiles = (int)((n_rows + SORT_TILE - 1) / SORT_TILE);
+  if (P.n_tiles < 1) P.n_tiles = 1;
+  P.buf[0] = reinterpret_cast<uint64_t*>(w + L.buf0);
+  P.buf[1] = reinterpret_cast<uint64_t*>(w + L.buf1);
+  P.state = reinterpret_cast<ColState*>(w + L.state);
+  P.tile_hist = reinterpret_cast<uint32_t*>(w + L.tile_hist);
+  uint32_t* totals = reinterpret_cast<uint32_t*>(w + L.totals);
+  key_sort_init_kernel<<<1, 1, 0, st>>>(P.state, n_rows);
+  ANV_CUDA(cudaGetLastError());
+  if (n_rows == 0) return ANV_OK;
+  for (int pass = first_pass; pass < end_pass; ++pass) {
+    P.pass = pass;
+    sort_hist_kernel<uint64_t><<<dim3((P.n_tiles + HIST_TPC - 1) / HIST_TPC, 1), ANV_BLOCK, 0, st>>>(P);
+    sort_totals_kernel<uint64_t><<<dim3(256, 1), ANV_BLOCK, 0, st>>>(P, totals);
+    sort_scan_kernel<uint64_t><<<dim3(256, 1), ANV_BLOCK, 0, st>>>(P, totals);
+    sort_scatter_kernel<uint64_t><<<dim3((P.n_tiles + SCAT_TPC - 1) / SCAT_TPC, 1), SCAT_THREADS, 0, st>>>(P);
+    ANV_CUDA(cudaGetLastError());
+  }
   return ANV_OK;
 }
 

@@ -1,12 +1,14 @@
 """Consumers of the stats hot path from `anovos.data_analyzer.quality_checker` (SURVEY.md 8f, row
 N2), same signatures and outputs as the reference
 (/root/reference/src/main/anovos/data_analyzer/quality_checker.py):
+  duplicate_detection   :49-149   (rows: hash, sort and exact comparison on the device - csrc/rows.cu)
+  nullRows_detection    :152-283  (rows: per-row null counts from the validity bitmaps - csrc/rows.cu)
   nullColumns_detection :286-547  (treatment: none / row_removal / column_removal)
   outlier_detection     :550-1045
   IDness_detection      :1048-1182
   biasedness_detection  :1185-1339
-Each returns (odf, odf_print).  The per-row work (null counts, distinct counts, modes, percentile /
-moment thresholds, the outlier compare pass) runs in the CUDA kernels.  Duplicate / invalid-entry
+Each returns (odf, odf_print) where the reference does.  The per-row work (row null counts, distinct rows, null counts,
+distinct counts, modes, percentile / moment thresholds, the outlier compare pass) runs in the CUDA kernels.  Invalid-entry
 detection and the imputation treatments (MMM / KNN / regression / MF / auto) are not part of this build."""
 from __future__ import annotations
 
@@ -57,6 +59,130 @@ def _read_stats(spec, columns):
         files = [path]
     df = pd.concat([pd.read_csv(f) if ftype == "csv" else pd.read_parquet(f) for f in files], ignore_index=True)
     return df[columns]
+
+
+# ---- row-level checks ----------------------------------------------------------------------------------
+
+def _row_cols(fr, list_of_cols, drop_cols):
+    """reference :103-114 / :224-235: "all" = numeric + categorical; an unknown name or an empty list is an error."""
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        num, cat, _ = attributeType_segregation(fr)
+        list_of_cols = num + cat
+    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    if any(c not in fr.columns for c in cols) or len(cols) == 0:
+        raise TypeError("Invalid input for Column(s)")
+    other = [c for c in cols if fr.column(c).kind == "other"]
+    if other:
+        raise TypeError("Column(s) %s have dtypes the GPU path does not hold (%s); row-level checks take numeric and "
+                        "string columns" % (",".join(other), ",".join(fr.column(c).sdtype for c in other)))
+    return cols
+
+
+def _canonical_codes(fr, cols):
+    """A frame whose string columns compare by code: a dictionary that repeats a string (a dictionary-typed Arrow input
+    can) has its codes mapped to the string's first code.  Other columns pass through untouched."""
+    out, changed = OrderedDict(), False
+    for c in cols:
+        col = fr.column(c)
+        dic = col.dictionary
+        if dic is not None and len(set(dic)) != len(dic):
+            torch = _lib.require_cuda()
+            first = {}
+            canon = np.array([first.setdefault(s, i) for i, s in enumerate(dic)], dtype=np.int32)
+            d, v = col.device()
+            lut = torch.from_numpy(canon).to(d.device)
+            codes = lut[d.long().clamp(0, len(dic) - 1)].to(torch.int32).contiguous()   # codes under null lanes are ignored
+            col = Column(c, col.sdtype, fr.n_rows, dev=codes, dev_valid=v, anv_dtype=_lib.ANV_I32, dictionary=dic)
+            changed = True
+        out[c] = col
+    return ColumnFrame(out, fr.n_rows) if changed else fr
+
+
+def duplicate_detection(spark, idf, list_of_cols="all", drop_cols=[], treatment=True, print_impact=False):
+    """reference :49-149.  Rows are grouped exactly on the device: a hash of each row's normalised values, an LSD sort of
+    (hash prefix, row) and a comparison of every row with its group's first row (csrc/rows.cu).  Nulls group together,
+    every NaN is one value and -0.0 == 0.0 (Spark 3 grouping).  The treated frame holds the `list_of_cols` columns of
+    the first occurrence of every distinct row, in row order (Spark's row and column order there is arbitrary)."""
+    fr = as_frame(idf)
+    if not treatment and not print_impact:
+        warnings.warn("The original idf will be the only output. Set print_impact=True to perform detection without treatment")
+        return fr
+    cols = _row_cols(fr, list_of_cols, drop_cols)
+    treatment = _as_bool(treatment, "treatment")
+    if getattr(fr, "is_partitioned", False):
+        raise NotImplementedError("duplicate_detection needs every row resident on one device to compare rows; "
+                                  "materialize() the row-partitioned frame first")
+    n = fr.count()
+    n_unique, first = engine.row_distinct(_canonical_codes(fr, cols), cols)
+    odf = fr.select(cols).filter_rows(engine.bitmap_to_bool(first, n)) if treatment else fr
+    if print_impact:
+        pct = round((n - n_unique) / n, 4)
+        odf_print = ResultFrame(pd.DataFrame([["rows_count", float(n)], ["unique_rows_count", float(n_unique)],
+                                              ["duplicate_rows", float(n - n_unique)], ["duplicate_pct", pct]],
+                                             columns=["metric", "value"]))
+        print("No. of Rows: " + str(n))
+        print("No. of UNIQUE Rows: " + str(n_unique))
+        print("No. of Duplicate Rows: " + str(n - n_unique))
+        print("Percentage of Duplicate Rows: " + str(pct))
+        return odf, odf_print
+    return odf
+
+
+def _null_rows_max_keep(n_cols, threshold):
+    """Largest null count that is NOT flagged: flagged when count > n_cols * threshold (product in Python float, as the
+    reference hands it to Spark), and at threshold 1 when count == n_cols (:255-264)."""
+    if threshold == 1:
+        return n_cols - 1
+    return min(int(math.floor(n_cols * threshold)), n_cols)
+
+
+def nullRows_detection(spark, idf, list_of_cols="all", drop_cols=[], treatment=False, treatment_threshold=0.8,
+                       print_impact=False):
+    """reference :152-283.  Per-row null counts come from the validity bitmaps on the device (csrc/rows.cu); NaN is a
+    value, not a null (the reference's UDF counts Python None).  A row-partitioned frame adds up the histograms of its
+    chunks (and of every rank of its process group); its treatment filters each chunk lazily."""
+    fr = as_frame(idf)
+    cols = _row_cols(fr, list_of_cols, drop_cols)
+    treatment = _as_bool(treatment, "treatment")
+    treatment_threshold = float(treatment_threshold)
+    if treatment_threshold < 0 or treatment_threshold > 1:
+        raise TypeError("Invalid input for Treatment Threshold Value")
+    max_keep = _null_rows_max_keep(len(cols), treatment_threshold)
+    n = fr.count()
+    odf = fr
+    if getattr(fr, "is_partitioned", False):
+        hist = np.zeros(len(cols) + 1, np.uint64)
+        kept = []
+        for ch in fr.chunks(cols):
+            h, _ = engine.row_null_counts(ch, cols)
+            hist += h
+            kept.append(int(h[:max_keep + 1].sum()) if max_keep >= 0 else 0)
+        if fr.group is not None:
+            hist = fr.group.all_reduce(hist)
+        if treatment:
+            def drop_flagged(ch):
+                _, keep = engine.row_null_counts(ch, cols, max_keep)
+                return ch.filter_rows(engine.bitmap_to_bool(keep, ch.n_rows))
+            odf = fr.map_chunks(fr._schema, drop_flagged)
+            odf.chunk_rows = kept
+            odf.n_rows_local = sum(kept)
+            odf.n_rows = odf.n_rows_local
+            if fr.group is not None:
+                odf.n_rows = int(fr.group.all_reduce(np.array([odf.n_rows_local], np.int64))[0])
+    else:
+        hist, keep = engine.row_null_counts(fr, cols, max_keep if treatment else None)
+        if treatment:
+            odf = fr.filter_rows(engine.bitmap_to_bool(keep, n))
+    ks = [k for k in range(len(cols) + 1) if int(hist[k]) > 0]
+    counts = [int(hist[k]) for k in ks]
+    flag = "treated" if treatment else "flagged"
+    odf_print = ResultFrame(pd.DataFrame({"null_cols_count": ks, "row_count": counts,
+                                          "row_pct": [spark_round(c / float(n)) for c in counts],
+                                          flag: [1 if k > max_keep else 0 for k in ks]},
+                                         columns=["null_cols_count", "row_count", "row_pct", flag]))
+    if print_impact:
+        odf_print.show(odf.count())
+    return odf, odf_print
 
 
 def nullColumns_detection(spark, idf, list_of_cols="missing", drop_cols=[], treatment=False, treatment_method="row_removal",

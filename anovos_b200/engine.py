@@ -493,6 +493,67 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
     return (out, rvals) if ranks is not None else out
 
 
+# ---- row-level checks ----------------------------------------------------------------------------
+
+def row_null_counts(frame: ColumnFrame, names, max_keep=None):
+    """-> (uint64 ndarray [len(names) + 1]: slot k = rows with k null columns among `names`,
+    int32 CUDA tensor of keep-bitmap words (bit set where the count <= max_keep) or None when max_keep is None).
+    Columns without a validity bitmap add nothing and are not handed to the kernel; the kernel reads the bitmaps only."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names = list(names)
+    ptrs, keepalive, nbytes = [], [], 0
+    for nme in names:
+        col = frame.column(nme)
+        if not col.has_validity:
+            continue
+        d, v = col.device()
+        if v is None:
+            continue
+        ptrs.append(v.data_ptr())
+        keepalive.append(v)
+        nbytes += (frame.n_rows + 7) // 8
+    dptrs = _to_dev(np.asarray(ptrs or [0], dtype=np.uint64))
+    counts = _dev_bytes((len(names) + 1) * 8)
+    keep = None
+    if max_keep is not None:
+        keep = torch.empty(max((frame.n_rows + 31) // 32, 1), dtype=torch.int32, device="cuda")
+    _call(L.anv_row_null_counts, "anv_row_null_counts", dptrs.data_ptr(), len(ptrs), len(names), frame.n_rows,
+          -1 if max_keep is None else int(max_keep), counts.data_ptr(), keep.data_ptr() if keep is not None else None,
+          _stream(), nbytes=nbytes if timer is not None else 0)
+    launch_count += 1
+    return _host(counts).view(np.uint64)[:len(names) + 1].copy(), keep
+
+
+def row_distinct(frame: ColumnFrame, names, hash_bits=0):
+    """-> (n_distinct, int32 CUDA tensor of first-occurrence bitmap words in row order).  Exact: rows are compared
+    after the hash sort, whatever the hash width (hash_bits 0 = the full width; small widths exercise the comparisons).
+    String columns compare by dictionary code: the caller maps repeated dictionary strings to one code first."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names = list(names)
+    if frame.n_rows >= (1 << 32):
+        raise _lib.AnvError("row_distinct: frames of 2^32 rows or more are not supported")
+    desc, keep = frame.descriptors(names) if names else (_dev_bytes(16), None)
+    ws_bytes = L.anv_row_distinct_workspace_bytes(frame.n_rows)
+    ws = _dev_bytes(ws_bytes)
+    nd = torch.zeros(1, dtype=torch.int64, device="cuda")
+    first = torch.empty(max((frame.n_rows + 31) // 32, 1), dtype=torch.int32, device="cuda")
+    _call(L.anv_row_distinct, "anv_row_distinct", desc.data_ptr(), len(names), frame.n_rows, int(hash_bits), nd.data_ptr(),
+          first.data_ptr(), ws.data_ptr(), ws_bytes, _stream(), nbytes=input_bytes(frame, names))
+    launch_count += 12
+    return int(nd.item()), first
+
+
+def bitmap_to_bool(words, n_rows):
+    """int32 bitmap words (LSB-first) on the device -> bool CUDA tensor [n_rows] (plumbing for frame.filter_rows)."""
+    torch = _lib.require_cuda()
+    rows = torch.arange(n_rows, device=words.device)
+    return ((words[rows >> 5] >> (rows & 31).to(torch.int32)) & 1).bool()
+
+
 # ---- HLL++ -------------------------------------------------------------------------------------
 
 _HLL_T = {4: 10, 5: 20, 6: 40, 7: 80, 8: 220, 9: 400, 10: 900, 11: 1800, 12: 3100, 13: 6500, 14: 11500,

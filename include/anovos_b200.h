@@ -216,6 +216,26 @@ int anv_mode_distinct_partition(const anv_column_t* cols, int n_cols, int64_t n_
                                 int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks, int n_ranks,
                                 double* rank_values, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- row null counts (nullRows_detection, quality_checker.py:248-272: a UDF counting None over the row's columns,
+ *      then groupBy(null_cols_count).count()).  validity [dev] n_bitmaps device pointers to the Arrow bitmaps of the
+ *      columns that HAVE one (a column without a bitmap adds nothing; n_cols counts every column and sizes `counts`).
+ *      NaN is not null.  counts [dev] n_cols + 1 uint64: slot k = rows with k null columns (zeroed by the library).
+ *      keep [dev] ceil(n_rows/32) bitmap words or NULL: bit set where the row's count <= max_keep (max_keep < 0: none). */
+int anv_row_null_counts(const uint32_t* const* validity, int n_bitmaps, int n_cols, int64_t n_rows, int max_keep,
+                        uint64_t* counts, uint32_t* keep, void* stream);
+
+/* ---- exact distinct rows (duplicate_detection, quality_checker.py:122-133: idf.groupby(list_of_cols).count()).
+ *      Rows are equal when every column is: null == null (the data under a null lane is ignored), every NaN equals
+ *      every NaN, -0.0 == 0.0, otherwise equal bits; string columns compare by dictionary code (the caller maps a
+ *      repeated dictionary string to one code).  Hash of each row -> LSD sort of (hash prefix, row) -> every row is
+ *      compared with its group's first row, so the result never depends on the hash being unique.
+ *      hash_bits caps the hash bits kept in the sort key (0 = all that fit above the row index; 1-8 send nearly every
+ *      row through the comparison path, for testing).  n_distinct [dev] 1 int64; first [dev] ceil(n_rows/32) bitmap
+ *      words, bit set on the first occurrence of every distinct row (row order).  n_rows >= 2^32: ANV_ERR_UNSUPPORTED. */
+size_t anv_row_distinct_workspace_bytes(int64_t n_rows);
+int anv_row_distinct(const anv_column_t* cols, int n_cols, int64_t n_rows, int hash_bits, int64_t* n_distinct,
+                     uint32_t* first, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- Spark's Bernoulli row sampler (the DEFAULT path of drift_detector.statistics: use_sampling=True ->
  *      data_sampling.py:122-149 `idf.sample(False, fraction, seed)` / `stat.sampleBy("merge", fractions, seed)`,
  *      drift_detector.py:187-211).  One partition per call: Spark seeds XORShiftRandom with seed + partitionIndex,
