@@ -68,6 +68,7 @@ _SIGNATURES = {
     "anv_mode_distinct_hll": (C.c_int, [_P, _I, _L, _I, _P, _P, _P, _P, _I, _P, _I, _P, _P, _SZ, _P]),
     "anv_mode_distinct_partition_workspace_bytes": (_SZ, [_I, _L]),
     "anv_mode_distinct_partition": (C.c_int, [_P, _I, _L, _P, _P, _P, _P, _I, _P, _P, _SZ, _P]),
+    "anv_mode_distinct_partition_hll": (C.c_int, [_P, _I, _L, _P, _P, _P, _P, _I, _P, _I, _P, _P, _SZ, _P]),
     "anv_row_null_counts": (C.c_int, [_P, _I, _I, _L, _I, _P, _P, _P]),
     "anv_row_distinct_workspace_bytes": (_SZ, [_L]),
     "anv_row_distinct": (C.c_int, [_P, _I, _L, _I, _P, _P, _P, _SZ, _P]),

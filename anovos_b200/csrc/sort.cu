@@ -1174,40 +1174,50 @@ int key_sort64(void* workspace, size_t workspace_bytes, int64_t n_rows, int firs
 
 
 // =====================================================================================================================
-// Partition + count path for 32-bit keys (F32 / I32 columns): what mode / distinct / percentiles need is the multiset of
-// keys in key ORDER, not a sorted array - so the columns are not sorted at all:
+// Two-level bucket count for 32-bit keys (F32 / I32 columns): what mode / distinct / percentiles / HLL++ need is the
+// multiset of keys grouped by value and a total order between groups, not a sorted array - so the columns are not sorted:
 //   sample     32 * P keys per column (stratified row positions), sorted with the LSD kernels above (tiny);
-//   split      P - 1 splitters = every 32nd sample key, plus the key of zero as a forced splitter, and a 4096-cell
-//              lookup table over the top 12 key bits that narrows the splitter search to a few steps;
-//   partition  ONE read of the raw column: every key finds its bucket (lower_bound over the splitters).  A key EQUAL to a
-//              splitter is only counted (warp-aggregated atomics) - any value frequent enough to unbalance a bucket is a
-//              splitter with overwhelming probability (it occupies >= 32 sample slots), so heavy hitters, exact zeros and
-//              discrete-valued columns never reach the key buffer; the other keys are appended to their bucket's slab
-//              (capacity 4x the mean bucket; the open 32-byte sectors of all buckets stay in L2 until they are full);
+//   split      P - 1 fine splitters = every 32nd sample key, plus the key of zero as a forced splitter (P = NS); every 32nd
+//              fine splitter is also a coarse splitter (G - 1 of them, G = P / 32 coarse groups of 32 fine splitters), with
+//              a 4096-cell lookup table over the top 12 key bits that narrows the coarse search to a few steps;
+//   coarse     fused into the pack step, ONE read of the raw column: per 4096-row tile, nulls dropped and zeros counted
+//              (as in pack_kernel), each key's coarse group found, the keys placed grouped by coarse group inside the tile
+//              (one shared-memory atomic per key: unstable, the order inside a group does not matter) and written
+//              coalesced to the tile's own range, with the (group, tile) counts in tile_hist's [256][n_tiles] shape;
+//   offsets    sort_totals / sort_scan over that table: every (group, tile) segment's offset in group-major order;
+//   fine       one CTA per chunk of <= 4096 consecutive group-major keys of one group: the chunk is gathered from its
+//              tile segments into shared memory, each key's fine bucket found among the group's 32 splitters (5 steps);
+//              keys EQUAL to a splitter are only counted (heavy hitters, discrete columns, NaN runs never move again), the
+//              others are written back in fine-bucket order into the chunk's own range of the second buffer, with the
+//              chunk's 34 bucket starts;
 //   cum        prefix sums over the interleaved (bucket, splitter) counts: total order of the column => every requested
-//              rank resolves to a splitter value directly or to (bucket, local rank);
-//   count      one CTA per bucket: shared-memory hash table key -> multiplicity (buckets larger than the table are swept
-//              several times, each sweep taking one hash class), distinct count and longest run per bucket, in-bucket radix
-//              select for the few buckets that hold a requested rank.
-// HBM traffic: one read of the column + ~1 write and 1 read of the keys that are not splitters (vs ~14 words per key for
-// the LSD path); no ranking, no stable scatter.  Counting is integer everywhere => deterministic results (the slab order is
-// not, and does not matter).  A bucket that overflows its slab or a hash table that fills up raises a per-column flag; the
-// host then redoes that column on the LSD path.
+//              rank resolves to a splitter value directly or to (bucket, local rank); splitters that occur add to the
+//              distinct count, the mode and the HLL++ registers once each;
+//   count      one CTA per (group, column) walks the group's fine buckets: each bucket's chunk segments are counted in a
+//              shared-memory hash table sized from the bucket's exact count (a larger bucket is swept by hash class), its
+//              distinct keys hashed once into shared-memory HLL++ registers, and the ranks that land in it selected.
+// Sizes are exact at every level: nothing is estimated, nothing overflows.  Global atomics happen once per (chunk,
+// bucket) or per (CTA, register), never per key.  HBM traffic: one read of the column + 4 words per key that is not a
+// splitter (written and read back twice) against ~14 for the LSD path; no ranking, no stable scatter.  Counting is
+// integer everywhere => deterministic results (the placement inside a group is not, and does not matter).
 constexpr uint32_t PC_ZERO_KEY = 0x80000000u;    // key of +-0.0 / integer 0: always a splitter, doubles as EMPTY in the hash table
 constexpr int PC_OVERSAMPLE = 32;
 constexpr int PC_LUT_BITS = 12;
 constexpr int PC_LUT_CELLS = 1 << PC_LUT_BITS;
+constexpr int PC_FPG = 32;                       // fine splitters per coarse group
+constexpr int PC_MAX_P = 8192;                   // => at most 256 coarse groups: the rows of the (group, tile) table
+constexpr int PC_CHUNK = 4096;                   // keys per fine-pass CTA
+constexpr int PC_CST = PC_FPG + 2;               // chunk table row: start of each of the 33 fine buckets + the end
+constexpr int PC_WIN = 512;                      // fine pass: tile segments located per round
+constexpr int PC_TPC = 16;                       // coarse pass: tiles per CTA (amortises the coarse splitters and table)
 constexpr int PC_SLOTS_LOG = 13;
 constexpr int PC_SLOTS = 1 << PC_SLOTS_LOG;      // hash table slots per CTA (64 KB: keys + counts)
-constexpr int PC_SWEEP_KEYS = 3072;              // keys one sweep of the table is sized for
-constexpr int PC_TILES_PER_CTA = 32;             // partition kernel: 32 x 4096 rows per CTA (amortises the splitter load)
+constexpr int PC_SWEEP_KEYS = 5120;              // keys one sweep of the table is sized for (<= 62.5 % load)
 constexpr int PC_MAX_RANKS = 16;
 
 struct PcCol {                     // per column, in the workspace (zeroed per call)
-  unsigned long long n_valid;      // non-null values
   unsigned long long distinct;     // sum of the buckets' distinct counts + splitters that occur
   unsigned long long best;         // max over (multiplicity << 32 | ~key): the mode, ties -> smallest key
-  int overflow;
   int n_queries;                   // ranks that fall inside a bucket
   int q_bucket[PC_MAX_RANKS];
   uint32_t q_local[PC_MAX_RANKS];  // 1-based rank inside the bucket
@@ -1218,16 +1228,27 @@ struct PcParams {
   const anv_column_t* cols;
   int n_cols;
   int64_t n_rows;
-  int P, NS, NB;                   // NS = P splitters (P - 1 from the sample + zero), NB = NS + 1 buckets
-  uint32_t cap;                    // slab capacity per bucket (keys)
+  int64_t stride;                  // keys per column in each key buffer
+  int n_tiles;
+  int P, NS, NB, G;                // NS = P splitters (P - 1 from the sample + zero), NB = NS + 1 buckets, G = P / 32 groups
+  int max_chunks;                  // fine chunks per column, upper bound: stride / PC_CHUNK + G
   int64_t m;                       // sample slots per column
   uint32_t* split;                 // [n_cols][NS]
-  uint16_t* lut;                   // [n_cols][PC_LUT_CELLS + 1]
-  uint32_t* cursor;                // [n_cols][NB]  keys appended to each bucket
-  uint32_t* cnt_eq;                // [n_cols][NS]  keys equal to each splitter
+  uint16_t* clut;                  // [n_cols][PC_LUT_CELLS + 1]  first coarse splitter >= each top-12-bit cell
+  uint32_t* keys[2];               // [n_cols][stride]  coarse output (per tile, grouped) / fine output (group-major)
+  ColState* state;                 // n_valid (nonzero keys) and n_zero per column, the scan's bookkeeping
+  uint32_t* tile_hist;             // [n_cols][256][n_tiles]  keys per (group, tile); after the scan: group-major offset
+  uint16_t* tile_start;            // [n_cols][256][n_tiles]  start of the group's keys inside the tile's range
+  uint32_t* totals;                // [n_cols][256]           keys per group
+  uint32_t* gstart;                // [n_cols][G + 1]         group-major offset of each group (+ the total)
+  uint32_t* chunk_base;            // [n_cols][G + 1]         first fine chunk of each group (+ the total)
+  uint16_t* cst;                   // [n_cols][max_chunks][PC_CST]  bucket starts inside each chunk's range
+  uint32_t* cnt_lt;                // [n_cols][NB]  keys strictly between two splitters, per bucket
+  uint32_t* cnt_eq;                // [n_cols][NS]  keys equal to each splitter (the zero run is added by pc_cum_kernel)
   uint32_t* cum;                   // [n_cols][2 * NB]  inclusive prefix over lt_0, eq_0, lt_1, eq_1, ...
-  uint32_t* slab;                  // [n_cols][NB][cap]
   PcCol* st;
+  int hll_p;                       // 0 = off
+  uint32_t* hll_regs;              // [n_cols][1 << hll_p]
 };
 
 template <typename T> __device__ __forceinline__ T load_elem(const void* base, int64_t row) {
@@ -1270,7 +1291,7 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_sample_kernel(const SortParams<u
   if (ok) S.buf[0][(size_t)c * S.stride + s_base + s_w[warp] + __popc(bal & ((1u << lane) - 1u))] = key;
 }
 
-// ---- split: splitters + lookup table of one column ---------------------------------------------------------------------
+// ---- split: fine splitters + the lookup table over the coarse ones, per column ---------------------------------------
 __global__ void __launch_bounds__(256) pc_split_kernel(const SortParams<uint32_t> S, const PcParams P) {
   const int c = blockIdx.x, tid = threadIdx.x;
   const ColState& st = S.state[c];
@@ -1290,130 +1311,277 @@ __global__ void __launch_bounds__(256) pc_split_kernel(const SortParams<uint32_t
   for (int j = tid; j < ns; j += 256) { const uint32_t v = sample_split(j); out[j < z ? j : j + 1] = v; }
   if (tid == 0) out[z] = PC_ZERO_KEY;
   __syncthreads();
-  uint16_t* lut = P.lut + (size_t)c * (PC_LUT_CELLS + 1);
+  // coarse splitter j = fine splitter 32 j + 31 (j < G - 1): a key's coarse group is the number of coarse splitters below it
+  uint16_t* lut = P.clut + (size_t)c * (PC_LUT_CELLS + 1);
+  const int nc = P.G - 1;
   for (int q = tid; q <= PC_LUT_CELLS; q += 256) {
-    int a = 0, b = P.NS;
-    if (q == PC_LUT_CELLS) { a = P.NS; }
+    int a = 0, b = nc;
+    if (q == PC_LUT_CELLS) { a = nc; }
     else {
       const uint32_t v = (uint32_t)q << (32 - PC_LUT_BITS);
-      while (a < b) { const int mid = (a + b) >> 1; if (out[mid] < v) a = mid + 1; else b = mid; }
+      while (a < b) { const int mid = (a + b) >> 1; if (out[mid * PC_FPG + PC_FPG - 1] < v) a = mid + 1; else b = mid; }
     }
     lut[q] = (uint16_t)a;
   }
 }
 
-// ---- partition ----------------------------------------------------------------------------------------------------------
+// ---- coarse: raw column -> keys grouped by coarse group inside each tile ------------------------------------------------
 template <typename T>
-__device__ __forceinline__ void pc_part_rows(const PcParams& P, const anv_column_t& col, const int c, const uint32_t* sS, const uint16_t* sL,
-                                             const int64_t r0, const int n_tile, unsigned long long& valid_acc) {
-  constexpr int VEC = 4, PER = SORT_TILE / ANV_BLOCK;
-  const int tid = threadIdx.x, lane = tid & 31;
-  const T* __restrict__ data = reinterpret_cast<const T*>(col.data) + r0;
-  const uint32_t* __restrict__ vbits = col.validity;
-  const int row0 = tid * PER;
-  uint32_t keys[PER];
-  uint32_t okmask = 0;
-  if (row0 + PER <= n_tile) {
-    uint32_t vb = 0xFFFFu;
-    if (vbits) { const int64_t g = r0 + row0; vb = (__ldg(vbits + (g >> 5)) >> (g & 31)) & 0xFFFFu; }
-    okmask = vb;
-    const uint4* p = reinterpret_cast<const uint4*>(data + row0);
+__device__ __forceinline__ void pc_coarse_tile(const PcParams& P, const anv_column_t& col, const int c, const int64_t tile,
+                                               const uint32_t* sC, const uint16_t* sL, uint32_t* hc, uint32_t* s_warp, uint32_t* sk,
+                                               uint32_t& n_zero, uint32_t& n_keys) {
+  constexpr int PER = SORT_TILE / ANV_BLOCK;        // 16 rounds of 256 rows (the strided pack: coalesced scalar loads)
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t r0 = tile * SORT_TILE;              // multiple of 4096: the tile starts on a bitmap word
+  const int n_tile = (int)min((int64_t)SORT_TILE, P.n_rows - r0);
+  const T* __restrict__ data = reinterpret_cast<const T*>(col.data) + r0 + tid;
+  const uint32_t* __restrict__ vw = col.validity ? col.validity + (r0 >> 5) + warp : nullptr;
+  const bool full = n_tile == SORT_TILE;
+  uint32_t wv = ANV_FULL;                           // lane i holds the warp's bitmap word of round i
+  if (vw && lane < PER && (full || lane * ANV_BLOCK + warp * 32 < n_tile)) wv = __ldg(vw + lane * (ANV_BLOCK / 32));
+  T x[PER];
 #pragma unroll
-    for (int v = 0; v < PER / VEC; ++v) {
-      const uint4 q = ldg_stream(p + v);
-      T e[VEC];
-      unpack<T>(q, e);
-#pragma unroll
-      for (int i = 0; i < VEC; ++i) keys[v * VEC + i] = make_key<uint32_t, T>(e[i]);
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < PER; ++i) {
-      const int row = row0 + i;
-      bool ok = row < n_tile;
-      keys[i] = 0;
-      if (ok) {
-        if (vbits) { const int64_t g = r0 + row; ok = (vbits[g >> 5] >> (g & 31)) & 1u; }
-        keys[i] = make_key<uint32_t, T>(data[row]);
-      }
-      okmask |= ok ? (1u << i) : 0u;
-    }
-  }
-  valid_acc += __popc(okmask);
-  uint32_t* __restrict__ cursor = P.cursor + (size_t)c * P.NB;
-  uint32_t* __restrict__ cnt_eq = P.cnt_eq + (size_t)c * P.NS;
-  uint32_t* __restrict__ slab = P.slab + (size_t)c * P.NB * P.cap;
-  bool over = false;
-#pragma unroll 4
   for (int i = 0; i < PER; ++i) {
-    const bool ok = (okmask >> i) & 1u;
-    const uint32_t k = keys[i];
-    int lo = sL[k >> (32 - PC_LUT_BITS)], hi = sL[(k >> (32 - PC_LUT_BITS)) + 1];
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (sS[mid] < k) lo = mid + 1; else hi = mid;
-    }
-    const bool eq = ok && lo < P.NS && sS[lo] == k;
-    const uint32_t em = __ballot_sync(ANV_FULL, eq);
-    if (eq) {
-      const uint32_t peers = __match_any_sync(em, lo);
-      if (lane == __ffs(peers) - 1) atomicAdd(&cnt_eq[lo], (uint32_t)__popc(peers));
-    } else if (ok) {
-      const uint32_t pos = atomicAdd(&cursor[lo], 1u);
-      if (pos < P.cap) slab[(size_t)lo * P.cap + pos] = k;
-      else over = true;
-    }
+    const bool in = full || (i * ANV_BLOCK + tid) < n_tile;
+    x[i] = in ? ld_stream_scalar<T>(data + i * ANV_BLOCK) : (T)0;
   }
-  if (over) P.st[c].overflow = 1;
-}
-
-__global__ void __launch_bounds__(ANV_BLOCK) pc_partition_kernel(const PcParams P) {
-  extern __shared__ __align__(16) uint32_t pc_sh[];
-  const int c = blockIdx.y, tid = threadIdx.x;
-  const anv_column_t col = P.cols[c];
-  uint32_t* sS = pc_sh;                                               // [NS]
-  uint16_t* sL = reinterpret_cast<uint16_t*>(pc_sh + ((P.NS + 3) & ~3));   // [PC_LUT_CELLS + 1]
-  {
-    const uint32_t* gS = P.split + (size_t)c * P.NS;
-    for (int i = tid; i < P.NS; i += ANV_BLOCK) sS[i] = gS[i];
-    const uint16_t* gL = P.lut + (size_t)c * (PC_LUT_CELLS + 1);
-    for (int i = tid; i <= PC_LUT_CELLS; i += ANV_BLOCK) sL[i] = gL[i];
+  uint32_t key[PER], slot[PER];                     // slot: group << 16 | rank inside the group, ~0 = no key
+#pragma unroll
+  for (int i = 0; i < PER; ++i) {
+    const uint32_t k = make_key<uint32_t, T>(x[i]);
+    bool ok = (__shfl_sync(ANV_FULL, wv, i) >> lane) & 1u;
+    if (!full) ok = ok && (i * ANV_BLOCK + tid) < n_tile;
+    const bool zero = ok && k == PC_ZERO_KEY;      // 0.0 and -0.0 share one key; integers: 0
+    n_zero += zero ? 1u : 0u;
+    ok = ok && !zero;
+    key[i] = k;
+    slot[i] = ~0u;
+    if (ok) {
+      const uint32_t q = k >> (32 - PC_LUT_BITS);
+      int lo = sL[q], hi = sL[q + 1];
+      while (lo < hi) { const int mid = (lo + hi) >> 1; if (sC[mid] < k) lo = mid + 1; else hi = mid; }
+      slot[i] = ((uint32_t)lo << 16) | atomicAdd(&hc[lo], 1u);
+    }
   }
   __syncthreads();
-  unsigned long long valid_acc = 0;
-  const int64_t first = (int64_t)blockIdx.x * PC_TILES_PER_CTA;
-  for (int t = 0; t < PC_TILES_PER_CTA; ++t) {
-    const int64_t r0 = (first + t) * SORT_TILE;
-    if (r0 >= P.n_rows) break;
-    const int n_tile = (int)min((int64_t)SORT_TILE, P.n_rows - r0);
-    if (col.dtype == ANV_F32) pc_part_rows<float>(P, col, c, sS, sL, r0, n_tile, valid_acc);
-    else pc_part_rows<int32_t>(P, col, c, sS, sL, r0, n_tile, valid_acc);
-  }
+  // exclusive scan of the 256 group counts (thread = group; groups >= G hold 0) -> the (group, tile) table
+  const uint32_t cnt = hc[tid];
+  uint32_t inc = cnt;
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) valid_acc += __shfl_down_sync(ANV_FULL, valid_acc, o);
-  if ((tid & 31) == 0 && valid_acc) atomicAdd(&P.st[c].n_valid, valid_acc);
+  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(ANV_FULL, inc, o); if (lane >= o) inc += t; }
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  uint32_t woff = 0, total = 0;
+#pragma unroll
+  for (int w = 0; w < ANV_WARPS; ++w) { const uint32_t t = s_warp[w]; woff += (w < warp) ? t : 0u; total += t; }
+  const uint32_t start = woff + inc - cnt;
+  const size_t row = ((size_t)c * 256 + tid) * P.n_tiles + tile;
+  P.tile_hist[row] = cnt;
+  P.tile_start[row] = (uint16_t)start;
+  hc[tid] = start;                                  // every thread read its own count above and nothing else
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < PER; ++i)
+    if (slot[i] != ~0u) sk[hc[slot[i] >> 16] + (slot[i] & 0xFFFFu)] = key[i];
+  __syncthreads();
+  uint32_t* __restrict__ out = P.keys[0] + (size_t)c * P.stride + r0;
+  for (uint32_t i = tid; i < total; i += ANV_BLOCK) out[i] = sk[i];
+  if (tid == 0) n_keys += total;
+  hc[tid] = 0;
+  __syncthreads();                                  // sk / hc / s_warp are reused by the CTA's next tile
+}
+
+__global__ void __launch_bounds__(ANV_BLOCK, 4) pc_coarse_kernel(const PcParams P) {
+  __shared__ uint32_t sC[PC_MAX_P / PC_FPG];
+  __shared__ uint16_t sL[PC_LUT_CELLS + 1];
+  __shared__ uint32_t hc[256], s_warp[ANV_WARPS];
+  __shared__ uint32_t sk[SORT_TILE];
+  const int c = blockIdx.y, tid = threadIdx.x;
+  const anv_column_t col = P.cols[c];
+  const uint32_t* S = P.split + (size_t)c * P.NS;
+  if (tid < P.G - 1) sC[tid] = S[tid * PC_FPG + PC_FPG - 1];
+  const uint16_t* L = P.clut + (size_t)c * (PC_LUT_CELLS + 1);
+  for (int i = tid; i <= PC_LUT_CELLS; i += ANV_BLOCK) sL[i] = L[i];
+  hc[tid] = 0;
+  __syncthreads();
+  uint32_t n_zero = 0, n_keys = 0;
+  for (int t = 0; t < PC_TPC; ++t) {
+    const int64_t tile = (int64_t)blockIdx.x * PC_TPC + t;
+    if (tile >= P.n_tiles) break;
+    if (col.dtype == ANV_F32) pc_coarse_tile<float>(P, col, c, tile, sC, sL, hc, s_warp, sk, n_zero, n_keys);
+    else pc_coarse_tile<int32_t>(P, col, c, tile, sC, sL, hc, s_warp, sk, n_zero, n_keys);
+  }
+  n_zero = __reduce_add_sync(ANV_FULL, n_zero);
+  if ((tid & 31) == 0 && n_zero) atomicAdd(&P.state[c].n_zero, (unsigned long long)n_zero);
+  if (tid == 0 && n_keys) atomicAdd(&P.state[c].n_valid, (unsigned long long)n_keys);
+}
+
+// ---- group starts and fine chunks per column (after the (group, tile) scan) -----------------------------------------------
+__global__ void __launch_bounds__(256) pc_chunks_kernel(const PcParams P) {
+  const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t t = tid < P.G ? P.totals[(size_t)c * 256 + tid] : 0u;
+  const uint32_t k = (t + PC_CHUNK - 1) / PC_CHUNK;
+  uint32_t it = t, ik = k;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t a = __shfl_up_sync(ANV_FULL, it, o), b = __shfl_up_sync(ANV_FULL, ik, o);
+    if (lane >= o) { it += a; ik += b; }
+  }
+  __shared__ uint32_t wt[8], wk[8];
+  if (lane == 31) { wt[warp] = it; wk[warp] = ik; }
+  __syncthreads();
+  uint32_t ot = 0, ok = 0, tt = 0, tk = 0;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) { ot += (w < warp) ? wt[w] : 0u; ok += (w < warp) ? wk[w] : 0u; tt += wt[w]; tk += wk[w]; }
+  uint32_t* gs = P.gstart + (size_t)c * (P.G + 1);
+  uint32_t* cb = P.chunk_base + (size_t)c * (P.G + 1);
+  if (tid < P.G) { gs[tid] = ot + it - t; cb[tid] = ok + ik - k; }
+  if (tid == 0) { gs[P.G] = tt; cb[P.G] = tk; }
+}
+
+// lower bound of k among the 32 sorted fine splitters of a group: 0..32 (32 only in the last group)
+__device__ __forceinline__ uint32_t pc_fine_bucket(const uint32_t* sF, uint32_t k) {
+  uint32_t f = (sF[15] < k) ? 16u : 0u;
+  f += (sF[f + 7] < k) ? 8u : 0u;
+  f += (sF[f + 3] < k) ? 4u : 0u;
+  f += (sF[f + 1] < k) ? 2u : 0u;
+  f += (sF[f] < k) ? 1u : 0u;
+  return f + ((f == 31u && sF[31] < k) ? 1u : 0u);
+}
+
+// ---- fine: one CTA per chunk of <= 4096 group-major keys -------------------------------------------------------------
+__global__ void __launch_bounds__(ANV_BLOCK) pc_fine_kernel(const PcParams P) {
+  const int c = blockIdx.y, b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t* cb = P.chunk_base + (size_t)c * (P.G + 1);
+  if ((uint32_t)b >= cb[P.G]) return;               // (uniform) the grid is sized for the largest possible chunk count
+  __shared__ uint32_t sk[PC_CHUNK], sk2[PC_CHUNK];
+  __shared__ uint32_t sO[PC_WIN + 1];
+  __shared__ uint16_t sTS[PC_WIN];
+  __shared__ uint32_t sF[PC_FPG], lc[PC_FPG + 1], ec[PC_FPG], ls[PC_CST];
+  __shared__ int s_g, s_t0;
+  const uint32_t* gs = P.gstart + (size_t)c * (P.G + 1);
+  if (warp == 0) {
+    int g = 0;
+    if (lane == 0) {                                // the group owning chunk b: last g with cb[g] <= b
+      int lo = 0, hi = P.G;
+      while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (cb[mid] <= (uint32_t)b) lo = mid; else hi = mid - 1; }
+      g = lo;
+    }
+    g = __shfl_sync(ANV_FULL, g, 0);
+    const uint32_t p0 = gs[g] + ((uint32_t)b - cb[g]) * PC_CHUNK;
+    // the tile whose segment holds p0: last t with O[t] <= p0, 32-ary search (O is non-decreasing over the tiles)
+    const uint32_t* O = P.tile_hist + ((size_t)c * 256 + g) * P.n_tiles;
+    int lo = 0, hi = P.n_tiles;
+    while (hi - lo > 1) {
+      const int step = (hi - lo + 31) / 32;
+      const int idx = lo + lane * step;
+      const uint32_t bal = __ballot_sync(ANV_FULL, idx < hi && O[idx] <= p0);   // lane 0 always: O[lo] <= p0
+      lo += (31 - __clz(bal)) * step;
+      hi = min(hi, lo + step);
+    }
+    if (lane == 0) { s_g = g; s_t0 = lo; }
+  }
+  if (tid < PC_FPG) ec[tid] = 0;
+  if (tid <= PC_FPG) lc[tid] = 0;
+  __syncthreads();
+  const int g = s_g;
+  const uint32_t gend = gs[g + 1];
+  const uint32_t p0 = gs[g] + ((uint32_t)b - cb[g]) * PC_CHUNK;
+  const uint32_t p1 = min(p0 + PC_CHUNK, gend);
+  const uint32_t* O = P.tile_hist + ((size_t)c * 256 + g) * P.n_tiles;
+  const uint16_t* TS = P.tile_start + ((size_t)c * 256 + g) * P.n_tiles;
+  const uint32_t* __restrict__ src = P.keys[0] + (size_t)c * P.stride;
+  if (tid < PC_FPG) sF[tid] = P.split[(size_t)c * P.NS + g * PC_FPG + tid];
+  // gather: the chunk's keys are the segments of consecutive tiles, in tile order; a round locates PC_WIN of them
+  for (int t0 = s_t0;; t0 += PC_WIN) {
+    for (int i = tid; i <= PC_WIN; i += ANV_BLOCK) {
+      const int t = t0 + i;
+      sO[i] = t < P.n_tiles ? O[t] : gend;
+      if (i < PC_WIN && t < P.n_tiles) sTS[i] = TS[t];
+    }
+    __syncthreads();
+    const uint32_t wlo = max(p0, sO[0]), whi = min(p1, sO[PC_WIN]);
+    for (uint32_t q = wlo + tid; q < whi; q += ANV_BLOCK) {
+      int lo = 0, hi = PC_WIN - 1;                  // last i with sO[i] <= q
+      while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (sO[mid] <= q) lo = mid; else hi = mid - 1; }
+      sk[q - p0] = src[(size_t)(t0 + lo) * SORT_TILE + sTS[lo] + (q - sO[lo])];
+    }
+    const bool done = whi >= p1;
+    __syncthreads();                                // sO / sTS are refilled by the next round
+    if (done) break;
+  }
+  // fine buckets: keys equal to a splitter are counted, the others ranked inside their bucket (unstable)
+  constexpr int PER = PC_CHUNK / ANV_BLOCK;
+  const uint32_t nk = p1 - p0;
+  uint32_t slot[PER];
+#pragma unroll
+  for (int r = 0; r < PER; ++r) {
+    const uint32_t i = tid + r * ANV_BLOCK;
+    slot[r] = ~0u;
+    if (i < nk) {
+      const uint32_t k = sk[i];
+      const uint32_t f = pc_fine_bucket(sF, k);
+      if (f < PC_FPG && sF[f] == k) atomicAdd(&ec[f], 1u);
+      else slot[r] = (f << 16) | atomicAdd(&lc[f], 1u);
+    }
+  }
+  __syncthreads();
+  if (warp == 0) {                                  // bucket starts inside the chunk: exclusive scan of lc[0..32]
+    const uint32_t v = lc[lane];
+    uint32_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(ANV_FULL, inc, o); if (lane >= o) inc += t; }
+    ls[lane] = inc - v;
+    if (lane == 31) { ls[32] = inc; ls[33] = inc + lc[32]; }
+  }
+  __syncthreads();
+  const int bucket0 = g * PC_FPG;
+  if (tid < PC_CST) P.cst[((size_t)c * P.max_chunks + b) * PC_CST + tid] = (uint16_t)ls[tid];
+  if (tid <= PC_FPG && lc[tid]) atomicAdd(&P.cnt_lt[(size_t)c * P.NB + bucket0 + tid], lc[tid]);
+  if (tid >= 64 && tid < 64 + PC_FPG && ec[tid - 64]) atomicAdd(&P.cnt_eq[(size_t)c * P.NS + bucket0 + tid - 64], ec[tid - 64]);
+#pragma unroll
+  for (int r = 0; r < PER; ++r)
+    if (slot[r] != ~0u) sk2[ls[slot[r] >> 16] + (slot[r] & 0xFFFFu)] = sk[tid + r * ANV_BLOCK];
+  __syncthreads();
+  uint32_t* __restrict__ out = P.keys[1] + (size_t)c * P.stride + p0;
+  const uint32_t n_out = ls[PC_CST - 1];
+  for (uint32_t i = tid; i < n_out; i += ANV_BLOCK) out[i] = sk2[i];
 }
 
 // ---- cum: total order of the column from the interleaved counts; rank queries; splitter contributions ---------------------
 __global__ void __launch_bounds__(1024) pc_cum_kernel(const PcParams P, const int64_t* ranks, const int n_ranks, double* rank_values) {
   const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   PcCol& st = P.st[c];
-  const uint32_t* cursor = P.cursor + (size_t)c * P.NB;
+  const uint32_t* cnt_lt = P.cnt_lt + (size_t)c * P.NB;
   const uint32_t* cnt_eq = P.cnt_eq + (size_t)c * P.NS;
   const uint32_t* S = P.split + (size_t)c * P.NS;
+  const uint32_t nz = (uint32_t)P.state[c].n_zero;       // the zero run never left the coarse pass: it is splitter PC_ZERO_KEY's
+  const int dt = P.cols[c].dtype;
   uint32_t* cum = P.cum + (size_t)c * 2 * P.NB;
   const int n_ent = 2 * P.NB - 1;                                     // lt_0, eq_0, lt_1, ..., eq_{NS-1}, lt_NS
   const int per = (n_ent + 1023) / 1024;
   const int e0 = tid * per, e1 = min(e0 + per, n_ent);
-  auto entry = [&](int e) -> uint32_t { return (e & 1) ? cnt_eq[e >> 1] : min(cursor[e >> 1], P.cap); };
+  auto entry = [&](int e) -> uint32_t {
+    if (!(e & 1)) return cnt_lt[e >> 1];
+    const int i = e >> 1;                                              // the zero run goes to the first splitter of zero
+    return cnt_eq[i] + ((S[i] == PC_ZERO_KEY && (i == 0 || S[i - 1] != PC_ZERO_KEY)) ? nz : 0u);
+  };
   unsigned long long run = 0, eq_distinct = 0, best = 0;
-  bool over = false;
   for (int e = e0; e < e1; ++e) {
-    run += entry(e);
-    if (e & 1) {
-      const uint32_t n = cnt_eq[e >> 1];
-      if (n) { ++eq_distinct; const unsigned long long cand = ((unsigned long long)n << 32) | (uint32_t)~S[e >> 1]; if (cand > best) best = cand; }
-    } else if (cursor[e >> 1] > P.cap) over = true;
+    const uint32_t n = entry(e);
+    run += n;
+    if ((e & 1) && n) {
+      const uint32_t k = S[e >> 1];
+      ++eq_distinct;
+      const unsigned long long cand = ((unsigned long long)n << 32) | (uint32_t)~k;
+      if (cand > best) best = cand;
+      if (P.hll_p) {
+        uint32_t idx, rho;
+        hll_slot(spark_hash_of_key<uint32_t>(k, dt), P.hll_p, idx, rho);
+        uint32_t* G = P.hll_regs + ((size_t)c << P.hll_p);
+        if (rho > G[idx]) atomicMax(&G[idx], rho);
+      }
+    }
   }
   __shared__ unsigned long long wsum[32];
   __shared__ unsigned long long wbest[32], wdist[32];
@@ -1428,7 +1596,6 @@ __global__ void __launch_bounds__(1024) pc_cum_kernel(const PcParams P, const in
   }
   if (lane == 31) wsum[warp] = inc;
   if (lane == 0) { wbest[warp] = rb; wdist[warp] = rd; }
-  if (over) st.overflow = 1;
   __syncthreads();
   if (warp == 0) {
     const unsigned long long w = wsum[lane];
@@ -1457,7 +1624,7 @@ __global__ void __launch_bounds__(1024) pc_cum_kernel(const PcParams P, const in
       int lo = 0, hi = n_ent - 1;
       while (lo < hi) { const int mid = (lo + hi) >> 1; if ((unsigned long long)cum[mid] < (unsigned long long)rk) lo = mid + 1; else hi = mid; }
       if (lo & 1) {
-        v = sorted_key_to_double((uint64_t)S[lo >> 1] << 32, P.cols[c].dtype);
+        v = sorted_key_to_double((uint64_t)S[lo >> 1] << 32, dt);
       } else {
         const int q = atomicAdd(&st.n_queries, 1);
         st.q_bucket[q] = lo >> 1;
@@ -1469,47 +1636,115 @@ __global__ void __launch_bounds__(1024) pc_cum_kernel(const PcParams P, const in
   }
 }
 
-// ---- count: one CTA per bucket ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(ANV_BLOCK) pc_count_kernel(const PcParams P, const int n_ranks, double* rank_values) {
-  const int c = blockIdx.y, b = blockIdx.x, tid = threadIdx.x;
-  PcCol& st = P.st[c];
-  const uint32_t n = min(P.cursor[(size_t)c * P.NB + b], P.cap);
-  if (n == 0) return;                                   // (uniform: the cursors are final when this kernel starts)
+// ---- count: one CTA per (group, column) walks the group's fine buckets ------------------------------------------------------
+// Visits the keys of fine bucket f of group g: warp w takes chunks w, w + 8, ... of the group, its lanes the chunk's segment.
+template <typename F>
+__device__ __forceinline__ void pc_for_bucket_keys(const PcParams& P, const int c, const int g, const int f, const uint32_t cb0,
+                                                   const uint32_t cb1, F&& fn) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint32_t* __restrict__ keys = P.keys[1] + (size_t)c * P.stride + P.gstart[(size_t)c * (P.G + 1) + g];
+  for (uint32_t j = cb0 + warp; j < cb1; j += ANV_WARPS) {
+    const uint16_t* row = P.cst + ((size_t)c * P.max_chunks + j) * PC_CST;
+    const uint32_t s = row[f], e = row[f + 1];
+    const uint32_t* __restrict__ base = keys + (size_t)(j - cb0) * PC_CHUNK;
+    for (uint32_t q = s + lane; q < e; q += 32) fn(base[q]);
+  }
+}
+
+__global__ void __launch_bounds__(ANV_BLOCK) pc_group_kernel(const PcParams P, const int n_ranks, double* rank_values) {
+  const int g = blockIdx.x, c = blockIdx.y, tid = threadIdx.x;
+  const uint32_t cb0 = P.chunk_base[(size_t)c * (P.G + 1) + g], cb1 = P.chunk_base[(size_t)c * (P.G + 1) + g + 1];
+  if (cb0 == cb1) return;                               // (uniform) no key between this group's splitters
   extern __shared__ __align__(16) uint32_t pc_tab[];
   uint32_t* tkey = pc_tab;
   uint32_t* tcnt = pc_tab + PC_SLOTS;
+  uint32_t* sreg = pc_tab + 2 * PC_SLOTS;               // [1 << hll_p] this CTA's HLL++ registers
   __shared__ uint32_t s_hist[256];
   __shared__ uint32_t s_sel[2];
-  const uint32_t* __restrict__ keys = P.slab + ((size_t)c * P.NB + b) * P.cap;
-  const uint32_t sweeps = (n + PC_SWEEP_KEYS - 1) / PC_SWEEP_KEYS;
+  __shared__ int s_full;
+  PcCol& st = P.st[c];
+  const int dt = P.cols[c].dtype;
+  const int hp = P.hll_p;
+  if (hp) for (int i = tid; i < (1 << hp); i += ANV_BLOCK) sreg[i] = 0;
   unsigned long long best = 0;
   uint32_t distinct = 0;
-  bool full = false;
-  for (uint32_t sw = 0; sw < sweeps; ++sw) {
-    for (int i = tid; i < PC_SLOTS; i += ANV_BLOCK) { tkey[i] = PC_ZERO_KEY; tcnt[i] = 0; }
-    __syncthreads();
-    for (uint32_t i = tid; i < n; i += ANV_BLOCK) {
-      const uint32_t k = keys[i];
-      if (sweeps > 1 && ((k * 0x85EBCA6Bu) >> 12) % sweeps != sw) continue;
-      uint32_t slot = (k * 0x9E3779B1u) >> (32 - PC_SLOTS_LOG);
-      int probes = 0;
-      while (true) {
-        const uint32_t prev = atomicCAS(&tkey[slot], PC_ZERO_KEY, k);
-        if (prev == PC_ZERO_KEY || prev == k) { atomicAdd(&tcnt[slot], 1u); break; }
-        slot = (slot + 1) & (PC_SLOTS - 1);
-        if (++probes >= PC_SLOTS) { full = true; break; }
+  const int nf = (g == P.G - 1) ? PC_FPG + 1 : PC_FPG;  // the last group also holds the keys above the top splitter
+  for (int f = 0; f < nf; ++f) {
+    const int bucket = g * PC_FPG + f;
+    const uint32_t n = P.cnt_lt[(size_t)c * P.NB + bucket];
+    if (n == 0) continue;                               // (uniform)
+    // hash classes: the top `lv` bits of k * odd (a bijection).  A class whose distinct keys do not fit the table is split in
+    // two; a class of 2^13 hash values holds at most 2^13 distinct keys, so the splitting stops by lv = 19.
+    int lv0 = 0;
+    while (((uint64_t)n >> lv0) > (uint64_t)PC_SWEEP_KEYS) ++lv0;
+    int tlog0 = 9;
+    while (tlog0 < PC_SLOTS_LOG && ((uint64_t)5 << tlog0) < (uint64_t)8 * min(n, (uint32_t)PC_SWEEP_KEYS)) ++tlog0;
+    int lv = lv0;
+    uint64_t lo = 0;                                    // first hash value of the current class
+    while (lo < (1ull << 32)) {
+      const int tlog = (lv == lv0) ? tlog0 : PC_SLOTS_LOG;
+      const uint32_t ts = 1u << tlog;
+      for (uint32_t i = tid; i < ts; i += ANV_BLOCK) { tkey[i] = PC_ZERO_KEY; tcnt[i] = 0; }
+      if (tid == 0) s_full = 0;
+      __syncthreads();
+      const uint32_t cls = lv ? (uint32_t)(lo >> (32 - lv)) : 0u;
+      pc_for_bucket_keys(P, c, g, f, cb0, cb1, [&](uint32_t k) {
+        if (lv && ((k * 0x85EBCA6Bu) >> (32 - lv)) != cls) return;
+        uint32_t slot = (k * 0x9E3779B1u) >> (32 - tlog);
+        for (uint32_t probes = 0; probes < ts; ++probes) {
+          const uint32_t prev = atomicCAS(&tkey[slot], PC_ZERO_KEY, k);
+          if (prev == PC_ZERO_KEY || prev == k) { atomicAdd(&tcnt[slot], 1u); return; }
+          slot = (slot + 1) & (ts - 1);
+        }
+        s_full = 1;
+      });
+      __syncthreads();
+      const int full = s_full;
+      __syncthreads();                                  // everyone has read s_full before the next class resets it
+      if (full) { ++lv; continue; }                     // (uniform) split this class and start over with its first half
+      for (uint32_t i = tid; i < ts; i += ANV_BLOCK) {
+        const uint32_t cnt = tcnt[i];
+        if (cnt) {
+          const uint32_t k = tkey[i];
+          ++distinct;
+          const unsigned long long cand = ((unsigned long long)cnt << 32) | (uint32_t)~k;
+          if (cand > best) best = cand;
+          if (hp) {
+            uint32_t idx, rho;
+            hll_slot(spark_hash_of_key<uint32_t>(k, dt), hp, idx, rho);
+            atomicMax(&sreg[idx], rho);
+          }
+        }
       }
+      __syncthreads();                                  // the table is cleared for the next class
+      lo += 1ull << (32 - lv);
+      while (lv > lv0 && (lo & ((1ull << (33 - lv)) - 1)) == 0) --lv;   // both halves done: back to the parent's level
     }
-    __syncthreads();
-    for (int i = tid; i < PC_SLOTS; i += ANV_BLOCK) {
-      const uint32_t cnt = tcnt[i];
-      if (cnt) {
-        ++distinct;
-        const unsigned long long cand = ((unsigned long long)cnt << 32) | (uint32_t)~tkey[i];
-        if (cand > best) best = cand;
+    // requested ranks inside this bucket: 4-pass radix select over the bucket's keys (L2-resident)
+    const int nq = st.n_queries;
+    for (int q = 0; q < nq; ++q) {
+      if (st.q_bucket[q] != bucket) continue;           // uniform across the CTA
+      uint32_t prefix = 0, r = st.q_local[q];
+      for (int pass = 3; pass >= 0; --pass) {
+        s_hist[tid] = 0;
+        __syncthreads();
+        const int sh = pass * 8;
+        pc_for_bucket_keys(P, c, g, f, cb0, cb1, [&](uint32_t k) {
+          if (pass == 3 || ((k ^ prefix) >> (sh + 8)) == 0) atomicAdd(&s_hist[(k >> sh) & 0xFFu], 1u);
+        });
+        __syncthreads();
+        if (tid == 0) {
+          uint32_t acc = 0, d = 0;
+          for (; d < 255; ++d) { if (acc + s_hist[d] >= r) break; acc += s_hist[d]; }
+          s_sel[0] = d; s_sel[1] = r - acc;
+        }
+        __syncthreads();
+        prefix |= s_sel[0] << sh;
+        r = s_sel[1];
+        __syncthreads();
       }
+      if (tid == 0) rank_values[(size_t)c * n_ranks + st.q_slot[q]] = sorted_key_to_double((uint64_t)prefix << 32, dt);
     }
-    __syncthreads();
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -1520,32 +1755,13 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_count_kernel(const PcParams P, c
     if (best) atomicMax(&st.best, best);
     if (distinct) atomicAdd(&st.distinct, (unsigned long long)distinct);
   }
-  if (full) st.overflow = 1;
-  // requested ranks inside this bucket: 4-pass radix select over the bucket's keys (L2-resident)
-  const int nq = st.n_queries;
-  for (int q = 0; q < nq; ++q) {
-    if (st.q_bucket[q] != b) continue;                     // uniform across the CTA
-    uint32_t prefix = 0, r = st.q_local[q];
-    for (int pass = 3; pass >= 0; --pass) {
-      s_hist[tid] = 0;
-      __syncthreads();
-      const int sh = pass * 8;
-      for (uint32_t i = tid; i < n; i += ANV_BLOCK) {
-        const uint32_t k = keys[i];
-        if (pass == 3 || ((k ^ prefix) >> (sh + 8)) == 0) atomicAdd(&s_hist[(k >> sh) & 0xFFu], 1u);
-      }
-      __syncthreads();
-      if (tid == 0) {
-        uint32_t acc = 0, d = 0;
-        for (; d < 255; ++d) { if (acc + s_hist[d] >= r) break; acc += s_hist[d]; }
-        s_sel[0] = d; s_sel[1] = r - acc;
-      }
-      __syncthreads();
-      prefix |= s_sel[0] << sh;
-      r = s_sel[1];
-      __syncthreads();
+  if (hp) {                                             // one global atomic per (CTA, register) that this CTA raised
+    __syncthreads();
+    uint32_t* G = P.hll_regs + ((size_t)c << hp);
+    for (int i = tid; i < (1 << hp); i += ANV_BLOCK) {
+      const uint32_t v = sreg[i];
+      if (v > G[i]) atomicMax(&G[i], v);
     }
-    if (tid == 0) rank_values[(size_t)c * n_ranks + st.q_slot[q]] = sorted_key_to_double((uint64_t)prefix << 32, P.cols[c].dtype);
   }
 }
 
@@ -1553,8 +1769,7 @@ __global__ void pc_final_kernel(const PcParams P, double* mode_value, int64_t* m
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= P.n_cols) return;
   const PcCol& st = P.st[c];
-  if (st.overflow) { mode_value[c] = nan(""); mode_rows[c] = -2; n_distinct[c] = -2; return; }   // redo on the LSD path
-  if (st.n_valid == 0 || st.best == 0) { mode_value[c] = nan(""); mode_rows[c] = 0; n_distinct[c] = 0; return; }
+  if (st.best == 0) { mode_value[c] = nan(""); mode_rows[c] = 0; n_distinct[c] = 0; return; }   // no non-null value
   const uint32_t key = ~(uint32_t)(st.best & 0xFFFFFFFFull);
   mode_value[c] = sorted_key_to_double((uint64_t)key << 32, P.cols[c].dtype);
   mode_rows[c] = (int64_t)(st.best >> 32);
@@ -1562,35 +1777,46 @@ __global__ void pc_final_kernel(const PcParams P, double* mode_value, int64_t* m
 }
 
 struct PcLayout {
-  int P, NS, NB;
-  uint32_t cap;
-  int64_t m;
-  size_t lsd, split, lut, cursor, cnt_eq, cum, st, slab, total;
+  int P, NS, NB, G, n_tiles, max_chunks;
+  int64_t m, stride;
+  size_t state, split, clut, cnt_lt, cnt_eq, cum, st, totals, gstart, chunk_base, lsd, keys0, keys1, tile_hist, tile_start, cst, total;
   PcLayout(int n_cols, int64_t n_rows) {
-    int p = 256;
-    while (p < 16384 && (int64_t)p * 3072 < n_rows) p <<= 1;
-    P = p; NS = p; NB = p + 1;
+    int p = 256;                                   // fine buckets of ~4096 rows
+    while (p < PC_MAX_P && (int64_t)p * SORT_TILE < n_rows) p <<= 1;
+    P = p; NS = p; NB = p + 1; G = p / PC_FPG;
     m = (int64_t)PC_OVERSAMPLE * p;
     if (m > n_rows) m = n_rows > 0 ? n_rows : 1;
-    const int64_t mean = n_rows / p + 1;
-    cap = (uint32_t)(((4 * mean + 1024) + 7) & ~(int64_t)7);
+    stride = (n_rows + 63) & ~(int64_t)63;
+    const int64_t nt = (n_rows + SORT_TILE - 1) / SORT_TILE;
+    n_tiles = nt > 0 ? (int)nt : 1;
+    max_chunks = (int)((stride + PC_CHUNK - 1) / PC_CHUNK) + G;
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t at = o; o = (o + bytes + 255) & ~(size_t)255; return at; };
-    lsd = take(Layout<uint32_t>(n_cols, m).total);
+    state = take((size_t)n_cols * sizeof(ColState));
     split = take((size_t)n_cols * NS * 4);
-    lut = take((size_t)n_cols * (PC_LUT_CELLS + 1) * 2);
-    cursor = take((size_t)n_cols * NB * 4);
+    clut = take((size_t)n_cols * (PC_LUT_CELLS + 1) * 2);
+    cnt_lt = take((size_t)n_cols * NB * 4);        // cnt_lt, cnt_eq, cum, st are contiguous: one memset
     cnt_eq = take((size_t)n_cols * NS * 4);
     cum = take((size_t)n_cols * 2 * NB * 4);
     st = take((size_t)n_cols * sizeof(PcCol));
-    slab = take((size_t)n_cols * NB * cap * 4);
-    total = o + 256;
+    totals = take((size_t)n_cols * 256 * 4);
+    gstart = take((size_t)n_cols * (G + 1) * 4);
+    chunk_base = take((size_t)n_cols * (G + 1) * 4);
+    // the sample sort's workspace is dead once the splitters are taken: it shares its space with the key buffers
+    lsd = o;
+    keys0 = take((size_t)n_cols * stride * 4);
+    keys1 = take((size_t)n_cols * stride * 4);
+    tile_hist = take((size_t)n_cols * 256 * n_tiles * 4);
+    tile_start = take((size_t)n_cols * 256 * n_tiles * 2);
+    cst = take((size_t)n_cols * max_chunks * PC_CST * 2);
+    const size_t sample_end = lsd + Layout<uint32_t>(n_cols, m).total;
+    total = (o > sample_end ? o : sample_end) + 256;
   }
 };
 
 static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_rows, double* mode_value, int64_t* mode_rows,
-                               int64_t* n_distinct, const int64_t* ranks, int n_ranks, double* rank_values, void* workspace,
-                               size_t workspace_bytes, cudaStream_t st) {
+                               int64_t* n_distinct, const int64_t* ranks, int n_ranks, double* rank_values, int hll_p,
+                               uint32_t* hll_regs, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   PcLayout L(n_cols, n_rows);
   if (workspace_bytes < L.total) { set_error("anv_mode_distinct_partition: workspace too small (%zu < %zu)", workspace_bytes, L.total); return ANV_ERR_WORKSPACE; }
   char* w = reinterpret_cast<char*>(workspace);
@@ -1607,52 +1833,68 @@ static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_r
   S.state = reinterpret_cast<ColState*>(ws + LS.state);
   S.tile_hist = reinterpret_cast<uint32_t*>(ws + LS.tile_hist);
   S.summ = reinterpret_cast<TileSummary<uint32_t>*>(ws + LS.summ);
-  uint32_t* totals = reinterpret_cast<uint32_t*>(ws + LS.totals);
+  uint32_t* sample_totals = reinterpret_cast<uint32_t*>(ws + LS.totals);
   PcParams P{};
-  P.cols = cols; P.n_cols = n_cols; P.n_rows = n_rows; P.P = L.P; P.NS = L.NS; P.NB = L.NB; P.cap = L.cap; P.m = L.m;
+  P.cols = cols; P.n_cols = n_cols; P.n_rows = n_rows; P.stride = L.stride; P.n_tiles = L.n_tiles;
+  P.P = L.P; P.NS = L.NS; P.NB = L.NB; P.G = L.G; P.max_chunks = L.max_chunks; P.m = L.m;
   P.split = reinterpret_cast<uint32_t*>(w + L.split);
-  P.lut = reinterpret_cast<uint16_t*>(w + L.lut);
-  P.cursor = reinterpret_cast<uint32_t*>(w + L.cursor);
+  P.clut = reinterpret_cast<uint16_t*>(w + L.clut);
+  P.keys[0] = reinterpret_cast<uint32_t*>(w + L.keys0);
+  P.keys[1] = reinterpret_cast<uint32_t*>(w + L.keys1);
+  P.state = reinterpret_cast<ColState*>(w + L.state);
+  P.tile_hist = reinterpret_cast<uint32_t*>(w + L.tile_hist);
+  P.tile_start = reinterpret_cast<uint16_t*>(w + L.tile_start);
+  P.totals = reinterpret_cast<uint32_t*>(w + L.totals);
+  P.gstart = reinterpret_cast<uint32_t*>(w + L.gstart);
+  P.chunk_base = reinterpret_cast<uint32_t*>(w + L.chunk_base);
+  P.cst = reinterpret_cast<uint16_t*>(w + L.cst);
+  P.cnt_lt = reinterpret_cast<uint32_t*>(w + L.cnt_lt);
   P.cnt_eq = reinterpret_cast<uint32_t*>(w + L.cnt_eq);
   P.cum = reinterpret_cast<uint32_t*>(w + L.cum);
   P.st = reinterpret_cast<PcCol*>(w + L.st);
-  P.slab = reinterpret_cast<uint32_t*>(w + L.slab);
+  P.hll_p = hll_regs ? hll_p : 0;
+  P.hll_regs = hll_regs;
+  // the (group, tile) table goes through the LSD path's totals / scan kernels
+  SortParams<uint32_t> T{};
+  T.cols = cols; T.n_cols = n_cols; T.n_rows = n_rows; T.stride = L.stride; T.n_tiles = L.n_tiles;
+  T.state = P.state; T.tile_hist = P.tile_hist; T.pass = 0;
+  if (hll_regs) ANV_CUDA(cudaMemsetAsync(hll_regs, 0, ((size_t)n_cols << hll_p) * sizeof(uint32_t), st));
   ANV_CUDA(cudaMemsetAsync(S.state, 0, (size_t)n_cols * sizeof(ColState), st));
-  ANV_CUDA(cudaMemsetAsync(w + L.cursor, 0, L.st + (size_t)n_cols * sizeof(PcCol) - L.cursor, st));   // cursor, cnt_eq, cum, st
+  ANV_CUDA(cudaMemsetAsync(P.state, 0, (size_t)n_cols * sizeof(ColState), st));
+  ANV_CUDA(cudaMemsetAsync(w + L.cnt_lt, 0, L.st + (size_t)n_cols * sizeof(PcCol) - L.cnt_lt, st));   // cnt_lt, cnt_eq, cum, st
   {
     dim3 grid((unsigned)((L.m + ANV_BLOCK - 1) / ANV_BLOCK), n_cols);
     pc_sample_kernel<<<grid, ANV_BLOCK, 0, st>>>(S, n_rows, L.m);
     ANV_CUDA(cudaGetLastError());
-    dim3 tg(S.n_tiles, n_cols);
     for (int pass = 0; pass < 4; ++pass) {
       S.pass = pass;
       sort_hist_kernel<uint32_t><<<dim3((S.n_tiles + HIST_TPC - 1) / HIST_TPC, n_cols), ANV_BLOCK, 0, st>>>(S);
-      sort_totals_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(S, totals);
-      sort_scan_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(S, totals);
+      sort_totals_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(S, sample_totals);
+      sort_scan_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(S, sample_totals);
       sort_scatter_kernel<uint32_t><<<dim3((S.n_tiles + SCAT_TPC - 1) / SCAT_TPC, n_cols), SCAT_THREADS, 0, st>>>(S);
       ANV_CUDA(cudaGetLastError());
     }
     pc_split_kernel<<<n_cols, 256, 0, st>>>(S, P);
     ANV_CUDA(cudaGetLastError());
   }
-  {
-    const size_t smem = (size_t)((L.NS + 3) & ~3) * 4 + (size_t)(PC_LUT_CELLS + 1) * 2 + 16;
-    static bool attr_done = false;
-    if (!attr_done) {
-      ANV_CUDA(cudaFuncSetAttribute(pc_partition_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-      ANV_CUDA(cudaFuncSetAttribute(pc_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PC_SLOTS * 8));
-      attr_done = true;
-    }
-    const int64_t tiles = (n_rows + SORT_TILE - 1) / SORT_TILE;
-    dim3 grid((unsigned)((tiles + PC_TILES_PER_CTA - 1) / PC_TILES_PER_CTA), n_cols);
-    if (tiles > 0) pc_partition_kernel<<<grid, ANV_BLOCK, smem, st>>>(P);
+  if (n_rows > 0) {
+    pc_coarse_kernel<<<dim3((L.n_tiles + PC_TPC - 1) / PC_TPC, n_cols), ANV_BLOCK, 0, st>>>(P);
+    sort_totals_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(T, P.totals);
+    sort_scan_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(T, P.totals);
+    pc_chunks_kernel<<<n_cols, 256, 0, st>>>(P);
+    pc_fine_kernel<<<dim3(L.max_chunks, n_cols), ANV_BLOCK, 0, st>>>(P);
     ANV_CUDA(cudaGetLastError());
   }
   pc_cum_kernel<<<n_cols, 1024, 0, st>>>(P, ranks, n_ranks, rank_values);
   ANV_CUDA(cudaGetLastError());
-  {
-    dim3 grid(L.NB, n_cols);
-    pc_count_kernel<<<grid, ANV_BLOCK, PC_SLOTS * 8, st>>>(P, n_ranks, rank_values);
+  if (n_rows > 0) {
+    const size_t smem = (size_t)PC_SLOTS * 8 + (P.hll_p ? ((size_t)4 << P.hll_p) : 0);
+    static bool attr_done = false;
+    if (!attr_done) {
+      ANV_CUDA(cudaFuncSetAttribute(pc_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PC_SLOTS * 8 + (4 << 12)));
+      attr_done = true;
+    }
+    pc_group_kernel<<<dim3(L.G, n_cols), ANV_BLOCK, smem, st>>>(P, n_ranks, rank_values);
     ANV_CUDA(cudaGetLastError());
   }
   pc_final_kernel<<<(n_cols + 127) / 128, 128, 0, st>>>(P, mode_value, mode_rows, n_distinct);
@@ -1697,15 +1939,24 @@ extern "C" size_t anv_mode_distinct_partition_workspace_bytes(int n_cols, int64_
   return PcLayout(n_cols, n_rows).total;
 }
 
-extern "C" int anv_mode_distinct_partition(const anv_column_t* cols, int n_cols, int64_t n_rows, double* mode_value,
-                                           int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks, int n_ranks,
-                                           double* rank_values, void* workspace, size_t workspace_bytes, void* stream) {
+extern "C" int anv_mode_distinct_partition_hll(const anv_column_t* cols, int n_cols, int64_t n_rows, double* mode_value,
+                                               int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks, int n_ranks,
+                                               double* rank_values, int hll_p, uint32_t* hll_regs, void* workspace,
+                                               size_t workspace_bytes, void* stream) {
   if (n_ranks < 0 || n_ranks > PC_MAX_RANKS || (n_ranks > 0 && (!ranks || !rank_values))) { set_error("anv_mode_distinct_partition: bad ranks arguments (n_ranks <= 16)"); return ANV_ERR_INVALID; }
   if (n_cols < 0 || n_rows < 0) { set_error("anv_mode_distinct_partition: bad arguments"); return ANV_ERR_INVALID; }
+  if (hll_regs && (hll_p < 4 || hll_p > 12)) { set_error("anv_mode_distinct_partition_hll: 4 <= hll_p <= 12"); return ANV_ERR_INVALID; }
   if (n_cols == 0) return ANV_OK;
   if (n_cols > 65535) { set_error("n_cols > 65535"); return ANV_ERR_UNSUPPORTED; }
   if (n_rows >= ((int64_t)1 << 32)) { set_error("anv_mode_distinct_partition: n_rows >= 2^32 per call is not supported"); return ANV_ERR_UNSUPPORTED; }
   if (!cols || !mode_value || !mode_rows || !n_distinct || !workspace) { set_error("anv_mode_distinct_partition: NULL argument"); return ANV_ERR_INVALID; }
-  return run_partition_count(cols, n_cols, n_rows, mode_value, mode_rows, n_distinct, ranks, n_ranks, rank_values, workspace,
-                             workspace_bytes, (cudaStream_t)stream);
+  return run_partition_count(cols, n_cols, n_rows, mode_value, mode_rows, n_distinct, ranks, n_ranks, rank_values, hll_p, hll_regs,
+                             workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int anv_mode_distinct_partition(const anv_column_t* cols, int n_cols, int64_t n_rows, double* mode_value,
+                                           int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks, int n_ranks,
+                                           double* rank_values, void* workspace, size_t workspace_bytes, void* stream) {
+  return anv_mode_distinct_partition_hll(cols, n_cols, n_rows, mode_value, mode_rows, n_distinct, ranks, n_ranks, rank_values, 0,
+                                         nullptr, workspace, workspace_bytes, stream);
 }

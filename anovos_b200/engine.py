@@ -383,8 +383,8 @@ def select_ranks(frame: ColumnFrame, names, ranks):
 # ---- sort-based exact mode / distinct --------------------------------------------------------
 
 SORT_WORKSPACE_BUDGET = 24 << 30  # bytes of scratch one sort batch may use
-sort_algorithm = "lsd"            # "lsd" | "partition" (32-bit columns through anv_mode_distinct_partition; tests run both)
-FUSED_HLL = True                  # sort_mode_distinct(..., hll_p=p) also returns the HLL++ registers (hashed from the sorted runs)
+sort_algorithm = "partition"      # "partition": F32 / I32 columns with <= 16 ranks take the bucket count; "lsd": every column sorts
+FUSED_HLL = True                  # sort_mode_distinct(..., hll_p=p) also returns the HLL++ registers (one hash per distinct value)
 
 
 def _mode_distinct_batch_size(frame, n_cols, per_col_bytes):
@@ -400,16 +400,15 @@ def _mode_distinct_batch_size(frame, n_cols, per_col_bytes):
 
 def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
     """-> list of (mode value | None, mode_rows | None, n_distinct) for NUMERIC columns.
-    hll_p (4..12, LSD path only): additionally returns the HyperLogLog++ registers uint32 [n_cols, 2**hll_p] as a by-product
-    of the run summaries (one hash per DISTINCT value instead of a separate pass over every value) - the result then is
+    hll_p (4..12): additionally returns the HyperLogLog++ registers uint32 [n_cols, 2**hll_p] as a by-product of the
+    counting (one hash per DISTINCT value instead of a separate pass over every value) - the result then is
     (list, rank values | None, registers).
     ranks: optional int64 [n_cols, n_ranks] of 1-based ranks among the non-null values (0 = skip);
     then returns (list, float64 [n_cols, n_ranks]) with the exact order statistics.
-    Default: the batched LSD radix sort (anv_mode_distinct).  sort_algorithm = "partition" sends 32-bit columns through
-    the partition + count path (anv_mode_distinct_partition: no sort, ~3 words of traffic per key, but its per-key global
-    atomics can make it slower than the sort - DESIGN.md section 3); a column that path hands back (mode_rows == -2)
-    is redone by the sort.  All column batches of a call are enqueued back to back on the stream into one workspace (stream
-    order makes the reuse safe) and the results come back in ONE device-to-host copy."""
+    F32 / I32 columns with at most 16 ranks go through the two-level bucket count (anv_mode_distinct_partition_hll: no
+    sort, ~4 words of traffic per key - DESIGN.md section 3); 64-bit columns, longer rank lists and sort_algorithm = "lsd"
+    take the batched LSD radix sort (anv_mode_distinct).  All column batches of a call are enqueued back to back on the
+    stream into one workspace (stream order makes the reuse safe) and the results come back in ONE device-to-host copy."""
     if getattr(frame, "is_partitioned", False):
         return frame.sort_mode_distinct(names, ranks)
     global launch_count
@@ -421,7 +420,7 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
         ranks = np.ascontiguousarray(ranks, dtype=np.int64).reshape(len(names), -1)
         n_ranks = ranks.shape[1]
     rvals = np.full((len(names), n_ranks), np.nan, np.float64)
-    want_hll = hll_p is not None and 4 <= hll_p <= 12 and sort_algorithm == "lsd"
+    want_hll = hll_p is not None and 4 <= hll_p <= 12
     hll_m = (1 << hll_p) if want_hll else 0
     hregs = np.zeros((len(names), hll_m), np.uint32) if want_hll else None
     res = {}
@@ -443,7 +442,7 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
         # one result block for the whole call: [mode_value | mode_rows | n_distinct | rank_values], 8 bytes per cell
         out = torch.empty((3 + n_ranks) * n_all, dtype=torch.int64, device="cuda")
         base = out.data_ptr()
-        dregs = torch.empty(max(n_all * hll_m, 1), dtype=torch.int32, device="cuda") if (want_hll and not partition) else None
+        dregs = torch.empty(max(n_all * hll_m, 1), dtype=torch.int32, device="cuda") if want_hll else None
         drk = _to_dev(ranks[idxs]) if n_ranks else None
         for b0 in range(0, n_all, batch):
             sub = [names[i] for i in idxs[b0:b0 + batch]]
@@ -453,9 +452,10 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
                       base + (3 * n_all + b0 * n_ranks) * 8 if n_ranks else None, ws.data_ptr(), ws_bytes, _stream())
             mv, mr, nd = base + b0 * 8, base + (n_all + b0) * 8, base + (2 * n_all + b0) * 8
             if partition:
-                _call(L.anv_mode_distinct_partition, "anv_mode_distinct_partition", desc.data_ptr(), n, frame.n_rows, mv, mr, nd,
-                      *common, nbytes=input_bytes(frame, sub))
-                launch_count += 6 + 16
+                _call(L.anv_mode_distinct_partition_hll, "anv_mode_distinct_partition", desc.data_ptr(), n, frame.n_rows, mv, mr,
+                      nd, *common[:3], hll_p if dregs is not None else 0,
+                      dregs.data_ptr() + b0 * hll_m * 4 if dregs is not None else None, *common[3:], nbytes=input_bytes(frame, sub))
+                launch_count += 11 + 16
             else:
                 _call(L.anv_mode_distinct_hll, "anv_mode_distinct", desc.data_ptr(), n, frame.n_rows, kb, mv, mr, nd,
                       *common[:3], hll_p if dregs is not None else 0,
@@ -469,24 +469,16 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
         if dregs is not None:
             hregs[np.asarray(idxs)] = _host(dregs.view(torch.uint8)).view(np.uint32)[:n_all * hll_m].reshape(n_all, hll_m)
         del ws
-        redo = []
         for j, i in enumerate(idxs):
             if hr[j] == -3:
                 raise _lib.AnvError("anv_mode_distinct: a one-sweep look-back gave up waiting for a preceding tile (column %r); "
                                     "unset ANV_SORT_ONESWEEP to use the three-kernel passes" % names[i])
-            if hr[j] == -2:               # a bucket overflowed (sampling failure): this column goes through the sort
-                redo.append(i)
-                continue
             if n_ranks:
                 rvals[i] = hrv[j]
             res[names[i]] = (float(hv[j]), int(hr[j]), int(hd[j])) if hr[j] > 0 else (None, None, 0)
-        return redo
 
     for kb, idxs in groups.items():
-        if kb == 32 and n_ranks <= 16 and sort_algorithm == "partition":
-            idxs = run(kb, idxs, True)
-        if idxs:
-            run(kb, idxs, False)
+        run(kb, idxs, kb == 32 and n_ranks <= 16 and sort_algorithm == "partition")
     out = [res[n] for n in names]
     if hll_p is not None:
         return out, (rvals if ranks is not None else None), hregs

@@ -206,12 +206,20 @@ int anv_mode_distinct_hll(const anv_column_t* cols, int n_cols, int64_t n_rows, 
                           int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks, int n_ranks, double* rank_values,
                           int hll_p, uint32_t* hll_regs, void* workspace, size_t workspace_bytes, void* stream);
 
-/* The same results for F32 / I32 columns WITHOUT sorting them (sort.cu, "partition + count"): sample -> splitters ->
- * one partition pass over the raw column (keys equal to a splitter - zeros, heavy hitters, discrete values - are only
- * counted) -> per-bucket shared-memory hash tables (multiplicities) and in-bucket radix select for the requested ranks.
- * About 3 words of HBM traffic per key instead of ~14.  A column whose bucket overflows (sampling failure; probability
- * negligible) comes back with mode_rows = n_distinct = -2: redo it with anv_mode_distinct.  n_ranks <= 16. */
+/* The same results - and, with hll_regs, the same HLL++ registers bit for bit - for F32 / I32 columns WITHOUT sorting
+ * them (sort.cu, "two-level bucket count"): sample -> fine splitters (every 32nd also a coarse one) -> the pack step groups
+ * every tile's keys by coarse group (one read of the raw column) -> one CTA per chunk of <= 4096 keys of a group moves them
+ * into fine-bucket order (keys equal to a splitter - zeros, heavy hitters, discrete values - are only counted) -> one CTA per
+ * group counts each fine bucket in a shared-memory hash table sized from its exact count, hashes its distinct keys into
+ * the HLL++ registers and selects the requested ranks that land in it.  About 4 words of HBM traffic per key instead of
+ * ~14; sizes are exact at every level, so nothing overflows.  n_ranks <= 16; 4 <= hll_p <= 12 (hll_regs NULL = off).
+ * The per-column workspace is no larger than anv_mode_distinct's for 32-bit keys from 65 536 rows up. */
 size_t anv_mode_distinct_partition_workspace_bytes(int n_cols, int64_t n_rows);
+int anv_mode_distinct_partition_hll(const anv_column_t* cols, int n_cols, int64_t n_rows, double* mode_value,
+                                    int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks, int n_ranks,
+                                    double* rank_values, int hll_p, uint32_t* hll_regs, void* workspace,
+                                    size_t workspace_bytes, void* stream);
+/* anv_mode_distinct_partition_hll without the registers. */
 int anv_mode_distinct_partition(const anv_column_t* cols, int n_cols, int64_t n_rows, double* mode_value,
                                 int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks, int n_ranks,
                                 double* rank_values, void* workspace, size_t workspace_bytes, void* stream);

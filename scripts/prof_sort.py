@@ -1,8 +1,11 @@
-"""Kernel breakdown of one sort_mode_distinct call (the LSD radix sort behind exact mode, distinct count, percentiles and
-HLL++ registers) at the default bench shape: the numeric columns of synth.device_frame(rows, cols, cat_every=4), with the
-summary ranks and hll_p the stats_generator step passes, so the column batching matches the step.
-torch.profiler with CUDA activities; prints ms per call for each kernel family, the card and its power limit, one JSON line.
-Usage: python scripts/prof_sort.py [rows] [cols] [calls] [tag]"""
+"""Kernel breakdown of one sort_mode_distinct call (exact mode, distinct count, percentiles and HLL++ registers) at the
+default bench shape: the numeric columns of synth.device_frame(rows, cols, cat_every=4), with the summary ranks and hll_p
+the stats_generator step passes, so the column batching matches the step.  algo: "partition" (the default two-level bucket
+count for 32-bit columns) or "lsd" (the radix sort for every column).
+torch.profiler with CUDA activities; prints ms per call for each kernel family next to the HBM bytes the family needs at
+these shapes (computed from the column sizes, not measured) and the rate that implies, the card and its power limit, and
+one JSON line.
+Usage: python scripts/prof_sort.py [rows] [cols] [calls] [tag] [algo]"""
 import collections
 import json
 import os
@@ -22,9 +25,13 @@ rows = int(float(sys.argv[1])) if len(sys.argv) > 1 else 40_000_000
 cols = int(sys.argv[2]) if len(sys.argv) > 2 else 200
 calls = int(sys.argv[3]) if len(sys.argv) > 3 else 2
 tag = sys.argv[4] if len(sys.argv) > 4 else "default"
+algo = sys.argv[5] if len(sys.argv) > 5 else "partition"
+engine.sort_algorithm = algo
 
 FAMILIES = ["pack_kernel", "sort_bases_kernel", "sort_hist_kernel", "sort_totals_kernel", "sort_scan_kernel",
-            "sort_scatter_kernel", "sort_onesweep_kernel", "run_tile_kernel", "run_merge_kernel"]
+            "sort_scatter_kernel", "sort_onesweep_kernel", "run_tile_kernel", "run_merge_kernel",
+            "pc_sample_kernel", "pc_split_kernel", "pc_coarse_kernel", "pc_chunks_kernel", "pc_fine_kernel", "pc_cum_kernel",
+            "pc_group_kernel", "pc_final_kernel", "pc_partition_kernel", "pc_count_kernel"]
 
 
 def family(name):
@@ -47,6 +54,14 @@ def card():
 fr = synth.device_frame(rows, cols, cat_every=4)
 num = [n for n in fr.columns if fr.column(n).kind == "num"]
 mom = engine.moments(fr, num)
+n_valid = np.array([int(mom["n_valid"][i]) for i in range(len(num))], dtype=np.int64)
+keys = int(np.array([int(mom["n_nonzero"][i]) for i in range(len(num))], dtype=np.int64).sum())   # nonzero non-null values
+raw = sum(fr.n_rows * 4 + (fr.n_rows + 7) // 8 * bool(fr.column(n).has_validity) for n in num)   # 32-bit columns + bitmaps
+# HBM bytes per family at these shapes (the keys equal to a fine splitter are counted as moved: an upper bound)
+if algo == "partition":
+    BYTES = {"pc_coarse": raw + 4 * keys, "pc_fine": 8 * keys, "pc_group": 4 * keys}
+else:
+    BYTES = {"pack": raw + 4 * keys, "hist": 4 * 4 * keys, "scatter": 4 * 8 * keys, "run_tile": 4 * keys}
 ranks = np.array([engine.quantile_ranks(int(mom["n_valid"][i]), anv_profile.SUMMARY_PROBS, anv_profile.SUMMARY_EPS)
                   for i in range(len(num))], dtype=np.int64)
 
@@ -75,9 +90,13 @@ for ev in trace["traceEvents"]:
         launches[f] += 1
 total = sum(ms.values())
 gpu, plim = card()
-print("%s, power limit %s; %d rows x %d numeric columns, per call:" % (gpu, plim, rows, len(num)))
+print("%s, power limit %s; %s path, %d rows x %d numeric columns, %.2f G nonzero keys, per call:"
+      % (gpu, plim, algo, rows, len(num), keys / 1e9))
 for f, t in sorted(ms.items(), key=lambda kv: -kv[1]):
-    print("  %-10s %8.2f ms  %5.1f %%  (%d launches per call)" % (f, t, 100 * t / total, launches[f] // calls))
-print("  %-10s %8.2f ms" % ("total", total))
-print(json.dumps({"tag": tag, "gpu": gpu, "power_limit": plim, "rows": rows, "numeric_cols": len(num), "calls": calls,
-                  "kernel_ms_per_call": round(total, 3), "ms_per_call": {f: round(t, 3) for f, t in ms.items()}}))
+    b = BYTES.get(f)
+    rate = ("  %6.1f GB  %6.0f GB/s" % (b / 1e9, b / 1e6 / t)) if b and t > 0 else ""
+    print("  %-12s %8.2f ms  %5.1f %%  (%d launches per call)%s" % (f, t, 100 * t / total, launches[f] // calls, rate))
+print("  %-12s %8.2f ms" % ("total", total))
+print(json.dumps({"tag": tag, "algo": algo, "gpu": gpu, "power_limit": plim, "rows": rows, "numeric_cols": len(num),
+                  "calls": calls, "kernel_ms_per_call": round(total, 3), "ms_per_call": {f: round(t, 3) for f, t in ms.items()},
+                  "hbm_gb": {f: round(b / 1e9, 2) for f, b in BYTES.items()}}))
