@@ -1193,8 +1193,9 @@ int key_sort64(void* workspace, size_t workspace_bytes, int64_t n_rows, int firs
 //   cum        prefix sums over the interleaved (bucket, splitter) counts: total order of the column => every requested
 //              rank resolves to a splitter value directly or to (bucket, local rank); splitters that occur add to the
 //              distinct count, the mode and the HLL++ registers once each;
-//   count      one CTA per (group, column) walks the group's fine buckets: each bucket's chunk segments are counted in a
-//              shared-memory hash table sized from the bucket's exact count (a larger bucket is swept by hash class), its
+//   count      one CTA per (group, column) walks the group's fine buckets: each bucket's chunk segments are copied into a
+//              shared-memory stage while the bucket before is counted, in a shared-memory hash table sized from the
+//              bucket's exact count (a bucket larger than the stage is streamed in pieces and swept by hash class), its
 //              distinct keys hashed once into shared-memory HLL++ registers, and the ranks that land in it selected.
 // Sizes are exact at every level: nothing is estimated, nothing overflows.  Global atomics happen once per (chunk,
 // bucket) or per (CTA, register), never per key.  HBM traffic: one read of the column + 4 words per key that is not a
@@ -1212,7 +1213,8 @@ constexpr int PC_WIN = 512;                      // fine pass: tile segments loc
 constexpr int PC_TPC = 16;                       // coarse pass: tiles per CTA (amortises the coarse splitters and table)
 constexpr int PC_SLOTS_LOG = 13;
 constexpr int PC_SLOTS = 1 << PC_SLOTS_LOG;      // hash table slots per CTA (64 KB: keys + counts)
-constexpr int PC_SWEEP_KEYS = 5120;              // keys one sweep of the table is sized for (<= 62.5 % load)
+constexpr int PC_SWEEP_KEYS = 5120;              // keys one sweep of the table is sized for (<= 62.5 % load), and of a stage
+constexpr int PC_GROUP_SMEM = PC_SLOTS * 8 + 2 * PC_SWEEP_KEYS * 4;   // count pass: table + 2 stage buffers, before HLL++
 constexpr int PC_MAX_RANKS = 16;
 
 struct PcCol {                     // per column, in the workspace (zeroed per call)
@@ -1242,7 +1244,7 @@ struct PcParams {
   uint32_t* totals;                // [n_cols][256]           keys per group
   uint32_t* gstart;                // [n_cols][G + 1]         group-major offset of each group (+ the total)
   uint32_t* chunk_base;            // [n_cols][G + 1]         first fine chunk of each group (+ the total)
-  uint16_t* cst;                   // [n_cols][max_chunks][PC_CST]  bucket starts inside each chunk's range
+  uint16_t* cst;                   // [n_cols][PC_CST][max_chunks]  bucket starts inside each chunk's range, bucket-major
   uint32_t* cnt_lt;                // [n_cols][NB]  keys strictly between two splitters, per bucket
   uint32_t* cnt_eq;                // [n_cols][NS]  keys equal to each splitter (the zero run is added by pc_cum_kernel)
   uint32_t* cum;                   // [n_cols][2 * NB]  inclusive prefix over lt_0, eq_0, lt_1, eq_1, ...
@@ -1439,6 +1441,13 @@ __global__ void __launch_bounds__(256) pc_chunks_kernel(const PcParams P) {
   if (tid == 0) { gs[P.G] = tt; cb[P.G] = tk; }
 }
 
+// 4-byte cp.async copies into shared memory: a thread issues all of its copies before it waits for any
+__device__ __forceinline__ void pc_cp_async4(uint32_t* dst, const uint32_t* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void pc_cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void pc_cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 // lower bound of k among the 32 sorted fine splitters of a group: 0..32 (32 only in the last group)
 __device__ __forceinline__ uint32_t pc_fine_bucket(const uint32_t* sF, uint32_t k) {
   uint32_t f = (sF[15] < k) ? 16u : 0u;
@@ -1504,12 +1513,15 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_fine_kernel(const PcParams P) {
     for (uint32_t q = wlo + tid; q < whi; q += ANV_BLOCK) {
       int lo = 0, hi = PC_WIN - 1;                  // last i with sO[i] <= q
       while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (sO[mid] <= q) lo = mid; else hi = mid - 1; }
-      sk[q - p0] = src[(size_t)(t0 + lo) * SORT_TILE + sTS[lo] + (q - sO[lo])];
+      pc_cp_async4(&sk[q - p0], src + (size_t)(t0 + lo) * SORT_TILE + sTS[lo] + (q - sO[lo]));   // nothing waits for it
     }
     const bool done = whi >= p1;
     __syncthreads();                                // sO / sTS are refilled by the next round
     if (done) break;
   }
+  pc_cp_commit();
+  pc_cp_wait<0>();
+  __syncthreads();
   // fine buckets: keys equal to a splitter are counted, the others ranked inside their bucket (unstable)
   constexpr int PER = PC_CHUNK / ANV_BLOCK;
   const uint32_t nk = p1 - p0;
@@ -1536,7 +1548,7 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_fine_kernel(const PcParams P) {
   }
   __syncthreads();
   const int bucket0 = g * PC_FPG;
-  if (tid < PC_CST) P.cst[((size_t)c * P.max_chunks + b) * PC_CST + tid] = (uint16_t)ls[tid];
+  if (tid < PC_CST) P.cst[((size_t)c * PC_CST + tid) * P.max_chunks + b] = (uint16_t)ls[tid];
   if (tid <= PC_FPG && lc[tid]) atomicAdd(&P.cnt_lt[(size_t)c * P.NB + bucket0 + tid], lc[tid]);
   if (tid >= 64 && tid < 64 + PC_FPG && ec[tid - 64]) atomicAdd(&P.cnt_eq[(size_t)c * P.NS + bucket0 + tid - 64], ec[tid - 64]);
 #pragma unroll
@@ -1637,90 +1649,117 @@ __global__ void __launch_bounds__(1024) pc_cum_kernel(const PcParams P, const in
 }
 
 // ---- count: one CTA per (group, column) walks the group's fine buckets ------------------------------------------------------
-// Visits the keys of fine bucket f of group g: warp w takes chunks w, w + 8, ... of the group, its lanes the chunk's segment.
-template <typename F>
-__device__ __forceinline__ void pc_for_bucket_keys(const PcParams& P, const int c, const int g, const int f, const uint32_t cb0,
-                                                   const uint32_t cb1, F&& fn) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t* __restrict__ keys = P.keys[1] + (size_t)c * P.stride + P.gstart[(size_t)c * (P.G + 1) + g];
-  for (uint32_t j = cb0 + warp; j < cb1; j += ANV_WARPS) {
-    const uint16_t* row = P.cst + ((size_t)c * P.max_chunks + j) * PC_CST;
-    const uint32_t s = row[f], e = row[f + 1];
-    const uint32_t* __restrict__ base = keys + (size_t)(j - cb0) * PC_CHUNK;
-    for (uint32_t q = s + lane; q < e; q += 32) fn(base[q]);
+// A bucket's keys are copied into a shared-memory stage with cp.async before they are counted, and the next bucket's copies
+// are issued before this one is counted: every thread keeps all of its copies in flight at once, and the count's shared
+// atomics never wait for HBM.
+struct PcCursor { uint32_t j, q; };  // next key of a bucket to stage: q keys into chunk j's segment (j = cb1: none left)
+
+struct PcStageScratch {              // one window of a bucket's segment list
+  uint32_t off[ANV_BLOCK], len[ANV_BLOCK], src[ANV_BLOCK];
+  uint32_t wsum[ANV_WARPS];
+  uint32_t cut_j, cut_q;
+};
+
+// Issues the copies of the next (at most PC_SWEEP_KEYS) keys of fine bucket f into dst and returns how many; `cur` moves
+// past them.  The segment list is walked ANV_BLOCK chunks at a time (a group can span thousands of chunks): thread t reads
+// chunk j + t's start and end (coalesced: cst is bucket-major), a block scan places the segments in the stage, and warp w
+// issues the copies of segments w, w + 8, ...  Nothing waits for the copies.  Every thread of the CTA calls it (barriers).
+__device__ uint32_t pc_stage_fill(const PcParams& P, const int c, const int f, const uint32_t* keys, const uint32_t cb0,
+                                  const uint32_t cb1, PcCursor& cur, uint32_t* dst, PcStageScratch& S) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint16_t* starts = P.cst + ((size_t)c * PC_CST + f) * P.max_chunks;   // + max_chunks: the segment ends
+  uint32_t n = 0;
+  while (cur.j < cb1 && n < PC_SWEEP_KEYS) {
+    const uint32_t j = cur.j + tid;
+    uint32_t s = 0, len = 0;
+    if (j < cb1) {
+      s = starts[j];
+      len = starts[j + P.max_chunks] - s;
+      if (tid == 0) { s += cur.q; len -= cur.q; }
+    }
+    uint32_t inc = len;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(ANV_FULL, inc, o); if (lane >= o) inc += t; }
+    if (lane == 31) S.wsum[warp] = inc;
+    __syncthreads();
+    uint32_t woff = 0, tot = 0;
+#pragma unroll
+    for (int w = 0; w < ANV_WARPS; ++w) { const uint32_t t = S.wsum[w]; woff += (w < warp) ? t : 0u; tot += t; }
+    const uint32_t off = n + woff + inc - len;       // the segment's place in the stage
+    S.off[tid] = off;
+    S.len[tid] = len;
+    S.src[tid] = (j - cb0) * PC_CHUNK + s;
+    if (len && off <= (uint32_t)PC_SWEEP_KEYS && (uint32_t)PC_SWEEP_KEYS < off + len) {   // the stage ends inside it
+      S.cut_j = j;
+      S.cut_q = (tid == 0 ? cur.q : 0u) + (PC_SWEEP_KEYS - off);
+    }
+    __syncthreads();
+    const uint32_t nwin = min(cb1 - cur.j, (uint32_t)ANV_BLOCK);
+    for (uint32_t t = warp; t < nwin; t += ANV_WARPS) {
+      const uint32_t o = S.off[t];
+      if (o >= (uint32_t)PC_SWEEP_KEYS) break;       // (uniform per warp) the offsets do not decrease
+      const uint32_t m = min(S.len[t], (uint32_t)PC_SWEEP_KEYS - o);
+      const uint32_t* from = keys + S.src[t];
+      for (uint32_t q = lane; q < m; q += 32) pc_cp_async4(dst + o + q, from + q);
+    }
+    if (n + tot <= (uint32_t)PC_SWEEP_KEYS) { n += tot; cur.j += nwin; cur.q = 0; }
+    else { n = PC_SWEEP_KEYS; cur.j = S.cut_j; cur.q = S.cut_q; }
+    __syncthreads();                                  // S is rewritten by the next window
   }
+  return n;
 }
 
-__global__ void __launch_bounds__(ANV_BLOCK) pc_group_kernel(const PcParams P, const int n_ranks, double* rank_values) {
+__global__ void __launch_bounds__(ANV_BLOCK, 2) pc_group_kernel(const PcParams P, const int n_ranks, double* rank_values) {
   const int g = blockIdx.x, c = blockIdx.y, tid = threadIdx.x;
   const uint32_t cb0 = P.chunk_base[(size_t)c * (P.G + 1) + g], cb1 = P.chunk_base[(size_t)c * (P.G + 1) + g + 1];
   if (cb0 == cb1) return;                               // (uniform) no key between this group's splitters
   extern __shared__ __align__(16) uint32_t pc_tab[];
   uint32_t* tkey = pc_tab;
   uint32_t* tcnt = pc_tab + PC_SLOTS;
-  uint32_t* sreg = pc_tab + 2 * PC_SLOTS;               // [1 << hll_p] this CTA's HLL++ registers
+  uint32_t* stage = pc_tab + 2 * PC_SLOTS;              // [2][PC_SWEEP_KEYS] two stage buffers
+  uint32_t* sreg = stage + 2 * PC_SWEEP_KEYS;           // [1 << hll_p] this CTA's HLL++ registers
+  __shared__ PcStageScratch S;
+  __shared__ uint32_t s_cnt[PC_FPG + 1];
   __shared__ uint32_t s_hist[256];
   __shared__ uint32_t s_sel[2];
   __shared__ int s_full;
   PcCol& st = P.st[c];
   const int dt = P.cols[c].dtype;
   const int hp = P.hll_p;
+  const uint32_t* __restrict__ keys = P.keys[1] + (size_t)c * P.stride + P.gstart[(size_t)c * (P.G + 1) + g];
+  const int nf = (g == P.G - 1) ? PC_FPG + 1 : PC_FPG;  // the last group also holds the keys above the top splitter
+  // the table is cleared once: every bucket and every sweep leaves the slots it used empty again
+  for (int i = tid; i < PC_SLOTS; i += ANV_BLOCK) { tkey[i] = PC_ZERO_KEY; tcnt[i] = 0; }
   if (hp) for (int i = tid; i < (1 << hp); i += ANV_BLOCK) sreg[i] = 0;
+  if (tid <= PC_FPG) s_cnt[tid] = tid < nf ? P.cnt_lt[(size_t)c * P.NB + g * PC_FPG + tid] : 0u;
+  if (tid == 0) s_full = 0;
+  __syncthreads();
   unsigned long long best = 0;
   uint32_t distinct = 0;
-  const int nf = (g == P.G - 1) ? PC_FPG + 1 : PC_FPG;  // the last group also holds the keys above the top splitter
-  for (int f = 0; f < nf; ++f) {
-    const int bucket = g * PC_FPG + f;
-    const uint32_t n = P.cnt_lt[(size_t)c * P.NB + bucket];
-    if (n == 0) continue;                               // (uniform)
-    // hash classes: the top `lv` bits of k * odd (a bijection).  A class whose distinct keys do not fit the table is split in
-    // two; a class of 2^13 hash values holds at most 2^13 distinct keys, so the splitting stops by lv = 19.
-    int lv0 = 0;
-    while (((uint64_t)n >> lv0) > (uint64_t)PC_SWEEP_KEYS) ++lv0;
-    int tlog0 = 9;
-    while (tlog0 < PC_SLOTS_LOG && ((uint64_t)5 << tlog0) < (uint64_t)8 * min(n, (uint32_t)PC_SWEEP_KEYS)) ++tlog0;
-    int lv = lv0;
-    uint64_t lo = 0;                                    // first hash value of the current class
-    while (lo < (1ull << 32)) {
-      const int tlog = (lv == lv0) ? tlog0 : PC_SLOTS_LOG;
-      const uint32_t ts = 1u << tlog;
-      for (uint32_t i = tid; i < ts; i += ANV_BLOCK) { tkey[i] = PC_ZERO_KEY; tcnt[i] = 0; }
-      if (tid == 0) s_full = 0;
-      __syncthreads();
-      const uint32_t cls = lv ? (uint32_t)(lo >> (32 - lv)) : 0u;
-      pc_for_bucket_keys(P, c, g, f, cb0, cb1, [&](uint32_t k) {
-        if (lv && ((k * 0x85EBCA6Bu) >> (32 - lv)) != cls) return;
-        uint32_t slot = (k * 0x9E3779B1u) >> (32 - tlog);
-        for (uint32_t probes = 0; probes < ts; ++probes) {
-          const uint32_t prev = atomicCAS(&tkey[slot], PC_ZERO_KEY, k);
-          if (prev == PC_ZERO_KEY || prev == k) { atomicAdd(&tcnt[slot], 1u); return; }
-          slot = (slot + 1) & (ts - 1);
-        }
-        s_full = 1;
-      });
-      __syncthreads();
-      const int full = s_full;
-      __syncthreads();                                  // everyone has read s_full before the next class resets it
-      if (full) { ++lv; continue; }                     // (uniform) split this class and start over with its first half
-      for (uint32_t i = tid; i < ts; i += ANV_BLOCK) {
-        const uint32_t cnt = tcnt[i];
-        if (cnt) {
-          const uint32_t k = tkey[i];
-          ++distinct;
-          const unsigned long long cand = ((unsigned long long)cnt << 32) | (uint32_t)~k;
-          if (cand > best) best = cand;
-          if (hp) {
-            uint32_t idx, rho;
-            hll_slot(spark_hash_of_key<uint32_t>(k, dt), hp, idx, rho);
-            atomicMax(&sreg[idx], rho);
-          }
-        }
-      }
-      __syncthreads();                                  // the table is cleared for the next class
-      lo += 1ull << (32 - lv);
-      while (lv > lv0 && (lo & ((1ull << (33 - lv)) - 1)) == 0) --lv;   // both halves done: back to the parent's level
+  auto fold = [&](uint32_t k, uint32_t cnt) {           // one distinct key of the bucket, with its multiplicity
+    ++distinct;
+    const unsigned long long cand = ((unsigned long long)cnt << 32) | (uint32_t)~k;
+    if (cand > best) best = cand;
+    if (hp) {
+      uint32_t idx, rho;
+      hll_slot(spark_hash_of_key<uint32_t>(k, dt), hp, idx, rho);
+      atomicMax(&sreg[idx], rho);
     }
-    // requested ranks inside this bucket: 4-pass radix select over the bucket's keys (L2-resident)
+  };
+  // counts k in the table's first 1 << tlog slots: its slot (claimed: k took an empty one), or ~0u when they are all taken
+  auto insert = [&](uint32_t k, int tlog, bool& claimed) -> uint32_t {
+    const uint32_t mask = (1u << tlog) - 1u;
+    uint32_t slot = (k * 0x9E3779B1u) >> (32 - tlog);
+    for (uint32_t probes = 0; probes <= mask; ++probes) {
+      const uint32_t prev = atomicCAS(&tkey[slot], PC_ZERO_KEY, k);
+      if (prev == PC_ZERO_KEY || prev == k) { atomicAdd(&tcnt[slot], 1u); claimed = prev == PC_ZERO_KEY; return slot; }
+      slot = (slot + 1) & mask;
+    }
+    claimed = false;
+    return ~0u;
+  };
+  // requested ranks inside a bucket: 4-pass radix select, each pass over the bucket's keys as each_key visits them
+  auto select = [&](const int bucket, auto&& each_key) {
     const int nq = st.n_queries;
     for (int q = 0; q < nq; ++q) {
       if (st.q_bucket[q] != bucket) continue;           // uniform across the CTA
@@ -1729,7 +1768,7 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_group_kernel(const PcParams P, c
         s_hist[tid] = 0;
         __syncthreads();
         const int sh = pass * 8;
-        pc_for_bucket_keys(P, c, g, f, cb0, cb1, [&](uint32_t k) {
+        each_key([&](uint32_t k) {
           if (pass == 3 || ((k ^ prefix) >> (sh + 8)) == 0) atomicAdd(&s_hist[(k >> sh) & 0xFFu], 1u);
         });
         __syncthreads();
@@ -1744,6 +1783,115 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_group_kernel(const PcParams P, c
         __syncthreads();
       }
       if (tid == 0) rank_values[(size_t)c * n_ranks + st.q_slot[q]] = sorted_key_to_double((uint64_t)prefix << 32, dt);
+    }
+  };
+  auto next_bucket = [&](int f) { do ++f; while (f < nf && s_cnt[f] == 0); return f; };
+  int buf = 0;                                          // stage buffer of the current bucket
+  bool staged = false;                                  // its copies were issued with the bucket before
+  for (int f = next_bucket(-1), fn; f < nf; f = fn) {
+    const int bucket = g * PC_FPG + f;
+    const uint32_t n = s_cnt[f];
+    fn = next_bucket(f);
+    if (n <= (uint32_t)PC_SWEEP_KEYS) {
+      // ---- the bucket fits the stage: counted from shared memory while the next one is copied into the other buffer
+      uint32_t* sk = stage + buf * PC_SWEEP_KEYS;
+      if (!staged) { PcCursor cu{cb0, 0}; pc_stage_fill(P, c, f, keys, cb0, cb1, cu, sk, S); pc_cp_commit(); }
+      staged = fn < nf && s_cnt[fn] <= (uint32_t)PC_SWEEP_KEYS;
+      if (staged) {
+        PcCursor cu{cb0, 0};
+        pc_stage_fill(P, c, fn, keys, cb0, cb1, cu, stage + (buf ^ 1) * PC_SWEEP_KEYS, S);
+        pc_cp_commit();
+        pc_cp_wait<1>();
+      } else {
+        pc_cp_wait<0>();
+      }
+      __syncthreads();
+      // one sweep: the table holds n keys at <= 62.5 % load, so it never fills up
+      int tlog = 9;
+      while (tlog < PC_SLOTS_LOG && (5u << tlog) < 8u * n) ++tlog;
+      uint32_t owned = 0;                               // bit r: this thread's key tid + r * ANV_BLOCK claimed a slot
+      for (uint32_t i = tid, r = 0; i < n; i += ANV_BLOCK, ++r) {
+        bool claimed;
+        const uint32_t slot = insert(sk[i], tlog, claimed);
+        if (claimed) { sk[i] = slot; owned |= 1u << r; }
+      }
+      __syncthreads();
+      while (owned) {                                   // each distinct key is folded by the thread that claimed its slot
+        const uint32_t i = tid + (__ffs(owned) - 1) * ANV_BLOCK;
+        owned &= owned - 1;
+        const uint32_t slot = sk[i], k = tkey[slot];
+        fold(k, tcnt[slot]);
+        tkey[slot] = PC_ZERO_KEY;
+        tcnt[slot] = 0;
+        sk[i] = k;                                      // the stage holds the bucket's keys again, for the select
+      }
+      __syncthreads();
+      select(bucket, [&](auto&& fn_key) { for (uint32_t i = tid; i < n; i += ANV_BLOCK) fn_key(sk[i]); });
+      buf ^= 1;
+    } else {
+      // ---- a larger bucket is streamed through both buffers in pieces, each piece copied while the one before is counted.
+      // Its keys are swept by hash classes, the top `lv` bits of k * odd (a bijection).  A class whose distinct keys do not
+      // fit the table is split in two; a class of 2^13 hash values holds at most 2^13 distinct keys, so the splitting
+      // stops by lv = 19.  Every sweep streams all the pieces again.
+      int lv0 = 0;
+      while ((n >> lv0) > (uint32_t)PC_SWEEP_KEYS) ++lv0;
+      int lv = lv0;
+      uint64_t lo = 0;                                  // first hash value of the current class
+      int b = 0;
+      PcCursor cu{cb0, 0};
+      uint32_t m_next = pc_stage_fill(P, c, f, keys, cb0, cb1, cu, stage, S);
+      pc_cp_commit();
+      while (true) {
+        const uint32_t cls = (uint32_t)(lo >> (32 - lv));
+        bool last;
+        do {
+          const uint32_t m = m_next;
+          last = cu.j >= cb1;
+          if (last) cu = PcCursor{cb0, 0};              // the piece after the last is the first again, for the next sweep
+          m_next = pc_stage_fill(P, c, f, keys, cb0, cb1, cu, stage + (b ^ 1) * PC_SWEEP_KEYS, S);
+          pc_cp_commit();
+          pc_cp_wait<1>();
+          __syncthreads();
+          const uint32_t* sk = stage + b * PC_SWEEP_KEYS;
+          for (uint32_t i = tid; i < m; i += ANV_BLOCK) {
+            const uint32_t k = sk[i];
+            if (((k * 0x85EBCA6Bu) >> (32 - lv)) != cls) continue;
+            bool claimed;
+            if (insert(k, PC_SLOTS_LOG, claimed) == ~0u) s_full = 1;
+          }
+          __syncthreads();                              // the buffer is refilled by the next piece
+          b ^= 1;
+        } while (!last);
+        const int full = s_full;
+        for (int i = tid; i < PC_SLOTS; i += ANV_BLOCK) {   // fold the class (unless it is split) and empty the table
+          const uint32_t cnt = tcnt[i];
+          if (cnt) {
+            if (!full) fold(tkey[i], cnt);
+            tkey[i] = PC_ZERO_KEY;
+            tcnt[i] = 0;
+          }
+        }
+        __syncthreads();                                // everyone has read s_full and the table is empty
+        if (tid == 0) s_full = 0;
+        if (full) { ++lv; continue; }                   // (uniform) split this class and start over with its first half
+        lo += 1ull << (32 - lv);
+        while (lv > lv0 && (lo & ((1ull << (33 - lv)) - 1)) == 0) --lv;   // both halves done: back to the parent's level
+        if (lo >= (1ull << 32)) break;
+      }
+      pc_cp_wait<0>();                                  // the first piece again, copied for a sweep that did not come
+      __syncthreads();
+      select(bucket, [&](auto&& fn_key) {
+        PcCursor sc{cb0, 0};
+        do {
+          const uint32_t m = pc_stage_fill(P, c, f, keys, cb0, cb1, sc, stage, S);
+          pc_cp_commit();
+          pc_cp_wait<0>();
+          __syncthreads();
+          for (uint32_t i = tid; i < m; i += ANV_BLOCK) fn_key(stage[i]);
+          __syncthreads();
+        } while (sc.j < cb1);
+      });
+      staged = false;
     }
   }
 #pragma unroll
@@ -1888,10 +2036,11 @@ static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_r
   pc_cum_kernel<<<n_cols, 1024, 0, st>>>(P, ranks, n_ranks, rank_values);
   ANV_CUDA(cudaGetLastError());
   if (n_rows > 0) {
-    const size_t smem = (size_t)PC_SLOTS * 8 + (P.hll_p ? ((size_t)4 << P.hll_p) : 0);
+    const size_t smem = (size_t)PC_GROUP_SMEM + (P.hll_p ? ((size_t)4 << P.hll_p) : 0);
     static bool attr_done = false;
-    if (!attr_done) {
-      ANV_CUDA(cudaFuncSetAttribute(pc_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PC_SLOTS * 8 + (4 << 12)));
+    if (!attr_done) {                               // sized for hll_p = 12; the carveout lets 2 CTAs share an SM at hll_p = 9
+      ANV_CUDA(cudaFuncSetAttribute(pc_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PC_GROUP_SMEM + (4 << 12)));
+      ANV_CUDA(cudaFuncSetAttribute(pc_group_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
       attr_done = true;
     }
     pc_group_kernel<<<dim3(L.G, n_cols), ANV_BLOCK, smem, st>>>(P, n_ranks, rank_values);

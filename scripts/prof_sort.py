@@ -4,8 +4,9 @@ the stats_generator step passes, so the column batching matches the step.  algo:
 count for 32-bit columns) or "lsd" (the radix sort for every column).
 torch.profiler with CUDA activities; prints ms per call for each kernel family next to the HBM bytes the family needs at
 these shapes (computed from the column sizes, not measured) and the rate that implies, the card and its power limit, and
-one JSON line.
-Usage: python scripts/prof_sort.py [rows] [cols] [calls] [tag] [algo]"""
+one JSON line.  hll_p = 0 leaves the HLL++ registers out and ranks = 0 the percentile ranks, so that a stage's time can
+be split into counting, hashing and selection.
+Usage: python scripts/prof_sort.py [rows] [cols] [calls] [tag] [algo] [hll_p] [ranks: 1 | 0]"""
 import collections
 import json
 import os
@@ -26,6 +27,8 @@ cols = int(sys.argv[2]) if len(sys.argv) > 2 else 200
 calls = int(sys.argv[3]) if len(sys.argv) > 3 else 2
 tag = sys.argv[4] if len(sys.argv) > 4 else "default"
 algo = sys.argv[5] if len(sys.argv) > 5 else "partition"
+hll_p = int(sys.argv[6]) if len(sys.argv) > 6 else anv_profile.DEFAULT_HLL_P
+with_ranks = (sys.argv[7] != "0") if len(sys.argv) > 7 else True
 engine.sort_algorithm = algo
 
 FAMILIES = ["pack_kernel", "sort_bases_kernel", "sort_hist_kernel", "sort_totals_kernel", "sort_scan_kernel",
@@ -67,7 +70,7 @@ ranks = np.array([engine.quantile_ranks(int(mom["n_valid"][i]), anv_profile.SUMM
 
 
 def run():
-    return engine.sort_mode_distinct(fr, num, ranks, hll_p=anv_profile.DEFAULT_HLL_P)
+    return engine.sort_mode_distinct(fr, num, ranks if with_ranks else None, hll_p=hll_p or None)
 
 
 run()                                   # warm-up: module load, workspace
@@ -90,13 +93,14 @@ for ev in trace["traceEvents"]:
         launches[f] += 1
 total = sum(ms.values())
 gpu, plim = card()
-print("%s, power limit %s; %s path, %d rows x %d numeric columns, %.2f G nonzero keys, per call:"
-      % (gpu, plim, algo, rows, len(num), keys / 1e9))
+print("%s, power limit %s; %s path, %d rows x %d numeric columns, %.2f G nonzero keys, hll_p %d, %s ranks, per call:"
+      % (gpu, plim, algo, rows, len(num), keys / 1e9, hll_p, "with" if with_ranks else "no"))
 for f, t in sorted(ms.items(), key=lambda kv: -kv[1]):
     b = BYTES.get(f)
     rate = ("  %6.1f GB  %6.0f GB/s" % (b / 1e9, b / 1e6 / t)) if b and t > 0 else ""
     print("  %-12s %8.2f ms  %5.1f %%  (%d launches per call)%s" % (f, t, 100 * t / total, launches[f] // calls, rate))
 print("  %-12s %8.2f ms" % ("total", total))
 print(json.dumps({"tag": tag, "algo": algo, "gpu": gpu, "power_limit": plim, "rows": rows, "numeric_cols": len(num),
+                  "hll_p": hll_p, "ranks": with_ranks,
                   "calls": calls, "kernel_ms_per_call": round(total, 3), "ms_per_call": {f: round(t, 3) for f, t in ms.items()},
                   "hbm_gb": {f: round(b / 1e9, 2) for f, b in BYTES.items()}}))
