@@ -1215,6 +1215,10 @@ constexpr int PC_SLOTS_LOG = 13;
 constexpr int PC_SLOTS = 1 << PC_SLOTS_LOG;      // hash table slots per CTA (64 KB: keys + counts)
 constexpr int PC_SWEEP_KEYS = 5120;              // keys one sweep of the table is sized for (<= 62.5 % load), and of a stage
 constexpr int PC_GROUP_SMEM = PC_SLOTS * 8 + 2 * PC_SWEEP_KEYS * 4;   // count pass: table + 2 stage buffers, before HLL++
+// Key values a direct bucket may span: 16-bit counters, two per word (32 KB).  2^15 covers a few % more keys but halves the
+// CTAs per SM; at c3 on H100 (700 W) the count stage took 34.8 ms at 2^14 and 42.3 ms at 2^15.
+constexpr int PC_DIRECT_RANGE = 1 << 14;
+constexpr int PC_DIRECT_SMEM = PC_DIRECT_RANGE * 2 + PC_SWEEP_KEYS * 4;   // direct count: counters + 1 stage, before HLL++
 constexpr int PC_MAX_RANKS = 16;
 
 struct PcCol {                     // per column, in the workspace (zeroed per call)
@@ -1709,17 +1713,37 @@ __device__ uint32_t pc_stage_fill(const PcParams& P, const int c, const int f, c
   return n;
 }
 
+// The one rule that splits the nonempty fine buckets between the two count kernels.  A bucket holds only keys strictly
+// between its neighbouring splitters lo and hi (lo = -1 below the first one, hi = 2^32 above the last), so it spans at
+// most R = hi - lo - 1 key values, known before anything is counted.  It is direct - counted by pc_direct_kernel in
+// 16-bit counters indexed by k - lo - 1 - when R <= PC_DIRECT_RANGE and its n keys fit a 16-bit counter; all other
+// buckets go to pc_group_kernel's hash table.  In float data a bucket of a few thousand keys spans few representable values.
+__device__ __forceinline__ bool pc_is_direct(const uint32_t* split, const int NS, const int bucket, const uint32_t n) {
+  const int64_t lo = bucket > 0 ? (int64_t)split[bucket - 1] : -1;
+  const int64_t hi = bucket < NS ? (int64_t)split[bucket] : (int64_t)1 << 32;
+  return n < (1u << 16) && hi - lo - 1 <= PC_DIRECT_RANGE;
+}
+
 __global__ void __launch_bounds__(ANV_BLOCK, 2) pc_group_kernel(const PcParams P, const int n_ranks, double* rank_values) {
   const int g = blockIdx.x, c = blockIdx.y, tid = threadIdx.x;
   const uint32_t cb0 = P.chunk_base[(size_t)c * (P.G + 1) + g], cb1 = P.chunk_base[(size_t)c * (P.G + 1) + g + 1];
   if (cb0 == cb1) return;                               // (uniform) no key between this group's splitters
+  const int nf = (g == P.G - 1) ? PC_FPG + 1 : PC_FPG;  // the last group also holds the keys above the top splitter
+  __shared__ uint32_t s_cnt[PC_FPG + 1];
+  uint32_t n_hash = 0;                                  // direct buckets count as empty here
+  if (tid < nf) {
+    const int bucket = g * PC_FPG + tid;
+    n_hash = P.cnt_lt[(size_t)c * P.NB + bucket];
+    if (pc_is_direct(P.split + (size_t)c * P.NS, P.NS, bucket, n_hash)) n_hash = 0;
+  }
+  if (tid <= PC_FPG) s_cnt[tid] = n_hash;
+  if (!__syncthreads_or(n_hash != 0)) return;           // (uniform) every bucket of the group is direct or empty
   extern __shared__ __align__(16) uint32_t pc_tab[];
   uint32_t* tkey = pc_tab;
   uint32_t* tcnt = pc_tab + PC_SLOTS;
   uint32_t* stage = pc_tab + 2 * PC_SLOTS;              // [2][PC_SWEEP_KEYS] two stage buffers
   uint32_t* sreg = stage + 2 * PC_SWEEP_KEYS;           // [1 << hll_p] this CTA's HLL++ registers
   __shared__ PcStageScratch S;
-  __shared__ uint32_t s_cnt[PC_FPG + 1];
   __shared__ uint32_t s_hist[256];
   __shared__ uint32_t s_sel[2];
   __shared__ int s_full;
@@ -1727,11 +1751,9 @@ __global__ void __launch_bounds__(ANV_BLOCK, 2) pc_group_kernel(const PcParams P
   const int dt = P.cols[c].dtype;
   const int hp = P.hll_p;
   const uint32_t* __restrict__ keys = P.keys[1] + (size_t)c * P.stride + P.gstart[(size_t)c * (P.G + 1) + g];
-  const int nf = (g == P.G - 1) ? PC_FPG + 1 : PC_FPG;  // the last group also holds the keys above the top splitter
   // the table is cleared once: every bucket and every sweep leaves the slots it used empty again
   for (int i = tid; i < PC_SLOTS; i += ANV_BLOCK) { tkey[i] = PC_ZERO_KEY; tcnt[i] = 0; }
   if (hp) for (int i = tid; i < (1 << hp); i += ANV_BLOCK) sreg[i] = 0;
-  if (tid <= PC_FPG) s_cnt[tid] = tid < nf ? P.cnt_lt[(size_t)c * P.NB + g * PC_FPG + tid] : 0u;
   if (tid == 0) s_full = 0;
   __syncthreads();
   unsigned long long best = 0;
@@ -1913,6 +1935,134 @@ __global__ void __launch_bounds__(ANV_BLOCK, 2) pc_group_kernel(const PcParams P
   }
 }
 
+// ---- direct count: one CTA per (group, column) walks the group's direct buckets (pc_is_direct) ------------------------------
+// Each key of a bucket bumps its own 16-bit counter, k - lo - 1, with a shared-memory add whose result nothing waits for:
+// no probing, no sweeps, one pass whatever the bucket's size.  A scan over the bucket's counters in key order then folds
+// each distinct key (multiplicity, mode, HLL++) and empties the counters again, so they are cleared once per CTA.  A count
+// never exceeds n < 2^16, so no carry reaches the neighbouring counter.
+__global__ void __launch_bounds__(ANV_BLOCK, 3) pc_direct_kernel(const PcParams P, const int n_ranks, double* rank_values) {
+  const int g = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t cb0 = P.chunk_base[(size_t)c * (P.G + 1) + g], cb1 = P.chunk_base[(size_t)c * (P.G + 1) + g + 1];
+  if (cb0 == cb1) return;                               // (uniform) no key between this group's splitters
+  const int nf = (g == P.G - 1) ? PC_FPG + 1 : PC_FPG;
+  const uint32_t* split = P.split + (size_t)c * P.NS;
+  __shared__ uint32_t s_cnt[PC_FPG + 1];                // keys of each direct bucket, 0 for the others
+  __shared__ uint32_t s_base[PC_FPG + 1];               // lo + 1: the key of the bucket's counter 0
+  __shared__ uint32_t s_range[PC_FPG + 1];              // R: the bucket's counters
+  uint32_t n_direct = 0;
+  if (tid < nf) {
+    const int bucket = g * PC_FPG + tid;
+    const uint32_t n = P.cnt_lt[(size_t)c * P.NB + bucket];
+    if (n && pc_is_direct(split, P.NS, bucket, n)) n_direct = n;
+    const uint32_t lo1 = bucket > 0 ? split[bucket - 1] + 1u : 0u;
+    s_base[tid] = lo1;
+    s_range[tid] = n_direct ? (bucket < P.NS ? split[bucket] : 0u) - lo1 : 0u;   // hi - lo - 1 (mod 2^32: hi = 2^32 -> 0)
+  }
+  if (tid <= PC_FPG) s_cnt[tid] = n_direct;
+  if (!__syncthreads_or(n_direct != 0)) return;         // (uniform) no direct bucket in this group
+  extern __shared__ __align__(16) uint32_t pc_dir[];
+  uint32_t* cw = pc_dir;                                // [PC_DIRECT_RANGE / 2] counter i in bits 16 (i & 1) of word i >> 1
+  uint32_t* stage = cw + PC_DIRECT_RANGE / 2;           // [PC_SWEEP_KEYS]
+  uint32_t* sreg = stage + PC_SWEEP_KEYS;               // [1 << hll_p] this CTA's HLL++ registers
+  __shared__ PcStageScratch S;
+  __shared__ uint32_t s_w[ANV_WARPS];
+  PcCol& st = P.st[c];
+  const int dt = P.cols[c].dtype;
+  const int hp = P.hll_p;
+  const uint32_t* __restrict__ keys = P.keys[1] + (size_t)c * P.stride + P.gstart[(size_t)c * (P.G + 1) + g];
+  uint4* cw4 = reinterpret_cast<uint4*>(cw);
+  for (int i = tid; i < PC_DIRECT_RANGE / 8; i += ANV_BLOCK) cw4[i] = make_uint4(0u, 0u, 0u, 0u);
+  if (hp) for (int i = tid; i < (1 << hp); i += ANV_BLOCK) sreg[i] = 0;
+  unsigned long long best = 0;
+  uint32_t distinct = 0;
+  const int nq = st.n_queries;
+  for (int f = 0; f < nf; ++f) {
+    if (s_cnt[f] == 0) continue;                        // (uniform)
+    const int bucket = g * PC_FPG + f;
+    const uint32_t base = s_base[f];
+    // ---- count: the bucket's segments are staged PC_SWEEP_KEYS keys at a time, all of a thread's copies in flight at once
+    PcCursor cu{cb0, 0};
+    do {                                                // pc_stage_fill's barriers order the last count / scan before its copies
+      const uint32_t m = pc_stage_fill(P, c, f, keys, cb0, cb1, cu, stage, S);
+      pc_cp_commit();
+      pc_cp_wait<0>();
+      __syncthreads();
+      for (uint32_t i = tid; i < m; i += ANV_BLOCK) {
+        const uint32_t d = stage[i] - base;
+        atomicAdd(&cw[d >> 1], 1u << ((d & 1u) << 4));
+      }
+    } while (cu.j < cb1);
+    __syncthreads();
+    // ---- ranks: first counter whose inclusive prefix reaches the local rank (threads own contiguous counter words)
+    for (int q = 0; q < nq; ++q) {
+      if (st.q_bucket[q] != bucket) continue;           // uniform across the CTA
+      constexpr int WPT = PC_DIRECT_RANGE / 2 / ANV_BLOCK;
+      static_assert((WPT & (WPT - 1)) == 0 && WPT >= 32, "the rotated reads need a power of two >= 32");
+      const uint32_t r = st.q_local[q];
+      uint32_t sum = 0;
+      for (int i = 0; i < WPT; ++i) {                   // each lane starts at its own word: no bank conflicts
+        const uint32_t w = cw[tid * WPT + ((i + lane) & (WPT - 1))];
+        sum += (w & 0xFFFFu) + (w >> 16);
+      }
+      uint32_t inc = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(ANV_FULL, inc, o); if (lane >= o) inc += t; }
+      if (lane == 31) s_w[warp] = inc;
+      __syncthreads();
+      uint32_t acc = inc - sum;
+      for (int w = 0; w < warp; ++w) acc += s_w[w];
+      if (acc < r && r <= acc + sum) {                  // exactly one thread holds the rank
+        uint32_t i = tid * WPT * 2;
+        for (;; ++i) {
+          acc += (cw[i >> 1] >> ((i & 1u) << 4)) & 0xFFFFu;
+          if (acc >= r) break;
+        }
+        rank_values[(size_t)c * n_ranks + st.q_slot[q]] = sorted_key_to_double((uint64_t)(base + i) << 32, dt);
+      }
+      __syncthreads();                                  // s_w is rewritten by the next query
+    }
+    // ---- scan: every nonzero counter is one distinct key, visited in key order; the words read are emptied again
+    const uint32_t nv = (s_range[f] + 7u) / 8u;
+    for (uint32_t v = tid; v < nv; v += ANV_BLOCK) {
+      const uint4 w4 = cw4[v];
+      if ((w4.x | w4.y | w4.z | w4.w) == 0u) continue;
+      cw4[v] = make_uint4(0u, 0u, 0u, 0u);
+      const uint32_t ws[4] = {w4.x, w4.y, w4.z, w4.w};
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const uint32_t cnt = (ws[e >> 1] >> ((e & 1) << 4)) & 0xFFFFu;
+        if (!cnt) continue;
+        const uint32_t k = base + 8u * v + (uint32_t)e;
+        ++distinct;
+        const unsigned long long cand = ((unsigned long long)cnt << 32) | (uint32_t)~k;
+        if (cand > best) best = cand;
+        if (hp) {
+          uint32_t idx, rho;
+          hll_slot(spark_hash_of_key<uint32_t>(k, dt), hp, idx, rho);
+          atomicMax(&sreg[idx], rho);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long ob = __shfl_down_sync(ANV_FULL, best, o); if (ob > best) best = ob;
+    distinct += __shfl_down_sync(ANV_FULL, distinct, o);
+  }
+  if ((tid & 31) == 0) {
+    if (best) atomicMax(&st.best, best);
+    if (distinct) atomicAdd(&st.distinct, (unsigned long long)distinct);
+  }
+  if (hp) {                                             // one global atomic per (CTA, register) that this CTA raised
+    __syncthreads();
+    uint32_t* G = P.hll_regs + ((size_t)c << hp);
+    for (int i = tid; i < (1 << hp); i += ANV_BLOCK) {
+      const uint32_t v = sreg[i];
+      if (v > G[i]) atomicMax(&G[i], v);
+    }
+  }
+}
+
 __global__ void pc_final_kernel(const PcParams P, double* mode_value, int64_t* mode_rows, int64_t* n_distinct) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= P.n_cols) return;
@@ -2044,6 +2194,15 @@ static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_r
       attr_done = true;
     }
     pc_group_kernel<<<dim3(L.G, n_cols), ANV_BLOCK, smem, st>>>(P, n_ranks, rank_values);
+    ANV_CUDA(cudaGetLastError());
+    const size_t dsmem = (size_t)PC_DIRECT_SMEM + (P.hll_p ? ((size_t)4 << P.hll_p) : 0);
+    static bool dattr_done = false;
+    if (!dattr_done) {                              // sized for hll_p = 12; 3 CTAs share an SM at hll_p = 9
+      ANV_CUDA(cudaFuncSetAttribute(pc_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PC_DIRECT_SMEM + (4 << 12)));
+      ANV_CUDA(cudaFuncSetAttribute(pc_direct_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+      dattr_done = true;
+    }
+    pc_direct_kernel<<<dim3(L.G, n_cols), ANV_BLOCK, dsmem, st>>>(P, n_ranks, rank_values);
     ANV_CUDA(cudaGetLastError());
   }
   pc_final_kernel<<<(n_cols + 127) / 128, 128, 0, st>>>(P, mode_value, mode_rows, n_distinct);

@@ -34,7 +34,7 @@ engine.sort_algorithm = algo
 FAMILIES = ["pack_kernel", "sort_bases_kernel", "sort_hist_kernel", "sort_totals_kernel", "sort_scan_kernel",
             "sort_scatter_kernel", "sort_onesweep_kernel", "run_tile_kernel", "run_merge_kernel",
             "pc_sample_kernel", "pc_split_kernel", "pc_coarse_kernel", "pc_chunks_kernel", "pc_fine_kernel", "pc_cum_kernel",
-            "pc_group_kernel", "pc_final_kernel", "pc_partition_kernel", "pc_count_kernel"]
+            "pc_group_kernel", "pc_direct_kernel", "pc_final_kernel", "pc_partition_kernel", "pc_count_kernel"]
 
 
 def family(name):
@@ -60,9 +60,11 @@ mom = engine.moments(fr, num)
 n_valid = np.array([int(mom["n_valid"][i]) for i in range(len(num))], dtype=np.int64)
 keys = int(np.array([int(mom["n_nonzero"][i]) for i in range(len(num))], dtype=np.int64).sum())   # nonzero non-null values
 raw = sum(fr.n_rows * 4 + (fr.n_rows + 7) // 8 * bool(fr.column(n).has_validity) for n in num)   # 32-bit columns + bitmaps
-# HBM bytes per family at these shapes (the keys equal to a fine splitter are counted as moved: an upper bound)
+# HBM bytes per family at these shapes (the keys equal to a fine splitter are counted as moved: an upper bound).  The count
+# stage reads every key once, split between pc_group (hash buckets) and pc_direct (direct buckets) by the data: its 4 bytes
+# per key are set against each kernel alone and against the two together ("count").
 if algo == "partition":
-    BYTES = {"pc_coarse": raw + 4 * keys, "pc_fine": 8 * keys, "pc_group": 4 * keys}
+    BYTES = {"pc_coarse": raw + 4 * keys, "pc_fine": 8 * keys, "pc_group": 4 * keys, "pc_direct": 4 * keys, "count": 4 * keys}
 else:
     BYTES = {"pack": raw + 4 * keys, "hist": 4 * 4 * keys, "scatter": 4 * 8 * keys, "run_tile": 4 * keys}
 ranks = np.array([engine.quantile_ranks(int(mom["n_valid"][i]), anv_profile.SUMMARY_PROBS, anv_profile.SUMMARY_EPS)
@@ -92,6 +94,8 @@ for ev in trace["traceEvents"]:
         ms[f] += ev["dur"] / 1e3 / calls
         launches[f] += 1
 total = sum(ms.values())
+if algo == "partition":
+    ms["count"] = ms["pc_group"] + ms["pc_direct"]   # not a kernel: left out of the total
 gpu, plim = card()
 print("%s, power limit %s; %s path, %d rows x %d numeric columns, %.2f G nonzero keys, hll_p %d, %s ranks, per call:"
       % (gpu, plim, algo, rows, len(num), keys / 1e9, hll_p, "with" if with_ranks else "no"))
@@ -99,6 +103,8 @@ for f, t in sorted(ms.items(), key=lambda kv: -kv[1]):
     b = BYTES.get(f)
     rate = ("  %6.1f GB  %6.0f GB/s" % (b / 1e9, b / 1e6 / t)) if b and t > 0 else ""
     print("  %-12s %8.2f ms  %5.1f %%  (%d launches per call)%s" % (f, t, 100 * t / total, launches[f] // calls, rate))
+    if f == "count":
+        print("  %-12s (pc_group + pc_direct, not in the total)" % "")
 print("  %-12s %8.2f ms" % ("total", total))
 print(json.dumps({"tag": tag, "algo": algo, "gpu": gpu, "power_limit": plim, "rows": rows, "numeric_cols": len(num),
                   "hll_p": hll_p, "ranks": with_ranks,
