@@ -70,6 +70,12 @@ __device__ __forceinline__ double sorted_key_to_double(uint64_t k, int dtype) {
   }
 }
 
+// The mode_value slot of a column: the value as a double, except for ANV_I64, whose slot holds the int64 itself, bit for
+// bit (a double holds only the int64s up to 2^53 exactly; the caller reads the slot as int64 for those columns).
+__device__ __forceinline__ double mode_slot_of_key(uint64_t k, int dtype) {
+  return dtype == ANV_I64 ? __longlong_as_double((long long)(k ^ (1ull << 63))) : sorted_key_to_double(k, dtype);
+}
+
 // Spark's hash of the VALUE a sorted key stands for (the HLL++ by-product of the run summaries): undo the order-preserving
 // transform; every NaN has the key ~0 and hashes as the canonical NaN, like Spark's floatToIntBits / doubleToLongBits.
 template <typename K> __device__ __forceinline__ uint64_t spark_hash_of_key(K k, int dtype);
@@ -972,7 +978,7 @@ __global__ void __launch_bounds__(32 * MERGE_WARPS) run_merge_kernel(const SortP
   }
   if (n == 0) {
     if (tid == 0) {
-      mode_value[c] = nz ? sorted_key_to_double(sizeof(K) == 8 ? (uint64_t)ZERO_KEY : ((uint64_t)ZERO_KEY << 32), dt) : nan("");
+      mode_value[c] = nz ? mode_slot_of_key(sizeof(K) == 8 ? (uint64_t)ZERO_KEY : ((uint64_t)ZERO_KEY << 32), dt) : nan("");
       mode_rows[c] = nz;
       n_distinct[c] = nz ? 1 : 0;
     }
@@ -1011,7 +1017,7 @@ __global__ void __launch_bounds__(32 * MERGE_WARPS) run_merge_kernel(const SortP
     if (acc.prefix_len != acc.n) best_of(bk, bl, acc.last_key, acc.suffix_len);
     int64_t rows = bl;
     if (nz > rows || (nz == rows && ZERO_KEY < bk)) { bk = ZERO_KEY; rows = nz; }   // ties: the smaller value
-    mode_value[c] = sorted_key_to_double(sizeof(K) == 8 ? (uint64_t)bk : ((uint64_t)bk << 32), dt);
+    mode_value[c] = mode_slot_of_key(sizeof(K) == 8 ? (uint64_t)bk : ((uint64_t)bk << 32), dt);
     mode_rows[c] = rows;
     n_distinct[c] = (int64_t)acc.heads_inside + 1 + (nz > 0 ? 1 : 0);
   }

@@ -419,6 +419,29 @@ def _outlier_cutoffs(param, detection_side):
     return [hi, lo], [-1, 0, 1]      # crossed bounds: a value between them is flagged by both sides: -1 + 1 = 0 (:952)
 
 
+def _outlier_thresholds_i64(param, detection_side):
+    """_outlier_cutoffs for a bigint column -> (cutoffs, flags of bins 1..len+1, exact int64 thresholds).  The reference
+    compares double(v) with the bounds (`v.astype(float)`, :937-950), so a bigint beyond 2^53 is rounded first: the flags
+    are `v <= T_lo` (<=> double(v) < lower) and `v > T_hi` (<=> double(v) > upper), with the exact integers
+    T_lo = the largest int64 whose double is < lower and T_hi = the largest whose double is <= upper (engine.i64_at_most).
+    NaN bounds flag nothing, like the reference's compare."""
+    lo = engine.i64_at_most(np.nextafter(param[0], -np.inf)) if param[0] is not None else None
+    hi = None if param[1] is None else (engine.I64_MAX if param[1] != param[1] else engine.i64_at_most(param[1]))
+    if detection_side == "lower":
+        ths, flags = [lo], [-1, 0]
+    elif detection_side == "upper":
+        ths, flags = [hi], [0, 1]
+    else:
+        ths, flags = sorted([lo, hi]), [-1, 0, 1]    # crossed bounds: as _outlier_cutoffs
+    # a threshold below -2^63 (no int64 qualifies) has an empty bin below it: clamp it to -2^63, and the values equal to
+    # -2^63, which then land in bin 1, take the flag of the first bin above every such threshold
+    k = sum(t < engine.I64_MIN for t in ths)
+    if k:
+        ths = [max(t, engine.I64_MIN) for t in ths]
+        flags = [flags[k]] + flags[1:]
+    return [float(t) for t in ths], flags, ths
+
+
 def outlier_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_side="upper", detection_configs=_OUTLIER_DEFAULTS,
                       treatment=True, treatment_method="value_replacement", pre_existing_model=False, model_path="NA",
                       sample_size=1000000, output_mode="replace", print_impact=False):
@@ -497,8 +520,9 @@ def outlier_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_si
     rows = []
     odf = fr
     if cols:
-        specs = [_outlier_cutoffs(p, detection_side) for p in params]
-        model = engine.BinModel(fr, cols, [s_[0] for s_ in specs])
+        specs = [_outlier_thresholds_i64(p, detection_side) if fr.column(c).anv_dtype == _lib.ANV_I64
+                 else _outlier_cutoffs(p, detection_side) + (None,) for c, p in zip(cols, params)]
+        model = engine.BinModel(fr, cols, [s_[0] for s_ in specs], exact=[s_[2] for s_ in specs])
         need_rows = treatment and not getattr(fr, "is_partitioned", False)
         if need_rows:
             ids = engine.bin_assign(fr, model)                        # [n_cols, n_rows] int32, 0 = null

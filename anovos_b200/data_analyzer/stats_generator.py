@@ -219,6 +219,8 @@ def _mode_str(col, value):
     if col.kind == "cat":
         return str(value)
     if col.sdtype in ("int", "bigint", "long"):
+        # Long.toString: the engine hands the mode of a bigint column over as an exact int, which int() keeps digit for
+        # digit (an int32 mode arrives as a float, which holds it exactly)
         return str(int(value))
     return jvm_double_str(float(value))
 

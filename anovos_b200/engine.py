@@ -156,18 +156,46 @@ def native_thresholds(cutoffs, anv_dtype) -> np.ndarray:
     return raw
 
 
-class BinModel:
-    """Host description of the binning of a set of columns + its device image."""
+I64_MIN, I64_MAX = -(1 << 63), (1 << 63) - 1
 
-    def __init__(self, frame: ColumnFrame, names, cutoffs, lo_hi=None):
+
+def i64_at_most(c) -> int:
+    """The largest int64 x whose double is <= c, as a Python int: `float(x) <= c` <=> `x <= i64_at_most(c)` for every int64
+    x, where float(x) is x rounded to the nearest double (ties to even), as NumPy's astype(float64) and the JVM's long ->
+    double conversion round.  I64_MIN - 1 when no int64 qualifies (c < -2^63, or NaN)."""
+    c = float(c)
+    if c != c or c < -2.0 ** 63:
+        return I64_MIN - 1
+    if c >= 2.0 ** 63:
+        return I64_MAX
+    x = math.floor(c)                       # exact: float(x) == x <= c
+    if x == c:                              # c is an integer: the ints up to the midpoint to the next double may round to c
+        nxt = math.nextafter(c, math.inf)
+        mid = x + (int(nxt) - x) // 2
+        x = mid if float(mid) <= c else mid - 1
+    return min(x, I64_MAX)
+
+
+class BinModel:
+    """Host description of the binning of a set of columns + its device image.
+    exact: optional per-column list of the native thresholds themselves, as Python ints (None: derive them from the
+    float64 cutoffs), for ANV_I64 columns whose thresholds a double cannot hold; value v goes to bin 1 + #(thresholds < v)."""
+
+    def __init__(self, frame: ColumnFrame, names, cutoffs, lo_hi=None, exact=None):
         self.names = list(names)
         self.cutoffs = [list(map(float, c)) for c in cutoffs]
+        self.exact = list(exact) if exact is not None else [None] * len(self.names)
         self.max_bins = max((len(c) + 1 for c in self.cutoffs), default=2)
         specs = np.zeros(len(self.names), dtype=_SPEC_DT)
         raws, off = [], 0
         for i, (nme, cut) in enumerate(zip(self.names, self.cutoffs)):
             col = frame.column(nme)
-            raw = native_thresholds(cut, col.anv_dtype)
+            if self.exact[i] is not None:
+                if col.anv_dtype != _lib.ANV_I64 or len(self.exact[i]) != len(cut):
+                    raise ValueError("exact thresholds are for bigint columns, one per cutoff (column %r)" % nme)
+                raw = np.array([int(t) for t in self.exact[i]], dtype=np.int64).view(np.uint64)   # out of range: OverflowError
+            else:
+                raw = native_thresholds(cut, col.anv_dtype)
             mode, lo, inv_w = 0, 0.0, 0.0
             if lo_hi is not None and lo_hi[i] is not None and col.anv_dtype in (_lib.ANV_F32, _lib.ANV_F64):
                 mn, mx = lo_hi[i]
@@ -399,7 +427,8 @@ def _mode_distinct_batch_size(frame, n_cols, per_col_bytes):
 
 
 def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
-    """-> list of (mode value | None, mode_rows | None, n_distinct) for NUMERIC columns.
+    """-> list of (mode value | None, mode_rows | None, n_distinct) for NUMERIC columns.  The mode of a bigint (ANV_I64)
+    column is an exact Python int, every other mode a float; rank values are float64 for every column, as in Spark.
     hll_p (4..12): additionally returns the HyperLogLog++ registers uint32 [n_cols, 2**hll_p] as a by-product of the
     counting (one hash per DISTINCT value instead of a separate pass over every value) - the result then is
     (list, rank values | None, registers).
@@ -463,6 +492,7 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
                 launch_count += 3 + 4 * (kb // 8)
         host = _host(out.view(torch.uint8))
         hv = host[:n_all * 8].view(np.float64)
+        hv64 = host[:n_all * 8].view(np.int64)        # the mode slot of an ANV_I64 column holds the int64 itself
         hr = host[n_all * 8:2 * n_all * 8].view(np.int64)
         hd = host[2 * n_all * 8:3 * n_all * 8].view(np.int64)
         hrv = host[3 * n_all * 8:].view(np.float64).reshape(n_all, n_ranks) if n_ranks else None
@@ -475,7 +505,11 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
                                     "unset ANV_SORT_ONESWEEP to use the three-kernel passes" % names[i])
             if n_ranks:
                 rvals[i] = hrv[j]
-            res[names[i]] = (float(hv[j]), int(hr[j]), int(hd[j])) if hr[j] > 0 else (None, None, 0)
+            if hr[j] <= 0:
+                res[names[i]] = (None, None, 0)
+                continue
+            mode = int(hv64[j]) if frame.column(names[i]).anv_dtype == _lib.ANV_I64 else float(hv[j])
+            res[names[i]] = (mode, int(hr[j]), int(hd[j]))
 
     for kb, idxs in groups.items():
         run(kb, idxs, kb == 32 and n_ranks <= 16 and sort_algorithm == "partition")

@@ -79,18 +79,20 @@ def gather_summaries_async(matrix: np.ndarray, n_max: int, device=None) -> Pendi
 
 def gather_summaries(matrix: np.ndarray, device=None):
     """all_gather of each rank's [n_local_cols, n_fields] summary matrix -> list over ranks.
-    Ranks may own different numbers of columns: matrices are padded to the largest."""
+    Ranks may own different numbers of columns: matrices are padded to the largest.  An int64 matrix is gathered as
+    int64 (exact 64-bit integers, e.g. the mode of a bigint column); anything else as float64."""
     import torch
     import torch.distributed as dist
     world = dist.get_world_size()
-    t = torch.from_numpy(np.ascontiguousarray(matrix, dtype=np.float64))
+    exact = np.asarray(matrix).dtype == np.int64
+    t = torch.from_numpy(np.ascontiguousarray(matrix, dtype=np.int64 if exact else np.float64))
     if device is not None:
         t = t.to(device)
     n_local = torch.tensor([t.shape[0]], dtype=torch.int64, device=t.device)
     counts = [torch.zeros_like(n_local) for _ in range(world)]
     dist.all_gather(counts, n_local)
     n_max = int(max(int(c.item()) for c in counts))
-    pad = torch.full((n_max, t.shape[1]), float("nan"), dtype=torch.float64, device=t.device)
+    pad = torch.full((n_max, t.shape[1]), 0 if exact else float("nan"), dtype=t.dtype, device=t.device)
     pad[:t.shape[0]] = t
     out = [torch.empty_like(pad) for _ in range(world)]
     dist.all_gather(out, pad)

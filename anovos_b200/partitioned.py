@@ -451,21 +451,34 @@ class PartitionedFrame:
         mine = block.columns
         n_ranks = 0 if ranks is None else np.asarray(ranks).reshape(len(names), -1).shape[1]
         rk = None if ranks is None else np.asarray(ranks, dtype=np.int64).reshape(len(names), -1)[[names.index(n) for n in mine]]
-        mat = np.zeros((len(mine), 3 + n_ranks), np.float64)
+        # [mode of a bigint column | mode_rows (-1: no value) | n_distinct] as int64, so a bigint mode stays exact;
+        # [mode of any other column | rank values] as float64
+        imat = np.zeros((len(mine), 3), np.int64)
+        fmat = np.full((len(mine), 1 + n_ranks), np.nan, np.float64)
         if mine:
             res = engine.sort_mode_distinct(block, mine, rk)
             modes, rvals = res if ranks is not None else (res, None)
             for i, (mv, mr, nd) in enumerate(modes):
-                mat[i, :3] = (np.nan if mv is None else mv, -1 if mr is None else mr, nd)
+                imat[i] = (mv if isinstance(mv, int) else 0, -1 if mr is None else mr, nd)
+                if isinstance(mv, float):
+                    fmat[i, 0] = mv
             if n_ranks:
-                mat[:, 3:] = rvals
-        full = np.concatenate(parallel.gather_summaries(mat, device="cuda" if self.group.device == "cuda" else None))
+                fmat[:, 1:] = rvals
+        dev = "cuda" if self.group.device == "cuda" else None
+        ifull = np.concatenate(parallel.gather_summaries(imat, device=dev))
+        ffull = np.concatenate(parallel.gather_summaries(fmat, device=dev))
         order = [n for r in range(self.group.world) for n in parallel.shard_columns(names, r, self.group.world)]
-        by = {n: full[i] for i, n in enumerate(order)}
-        out = [((float(by[n][0]), int(by[n][1]), int(by[n][2])) if by[n][1] >= 0 else (None, None, 0)) for n in names]
+        at = {n: i for i, n in enumerate(order)}
+        out = []
+        for n in names:
+            mv, mr, nd = (int(x) for x in ifull[at[n]])
+            if mr < 0:
+                out.append((None, None, 0))
+            else:
+                out.append((mv if self.column(n).anv_dtype == _lib.ANV_I64 else float(ffull[at[n], 0]), mr, nd))
         if ranks is None:
             return out
-        return out, np.array([by[n][3:] for n in names], dtype=np.float64).reshape(len(names), n_ranks)
+        return out, np.array([ffull[at[n], 1:] for n in names], dtype=np.float64).reshape(len(names), n_ranks)
 
 
 # ---- row slabs -> column blocks (the one real exchange step) ---------------------------------------

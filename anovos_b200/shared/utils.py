@@ -4,11 +4,12 @@ need (round HALF_UP, Double.toString)."""
 from __future__ import annotations
 
 import math
-from decimal import ROUND_HALF_UP, Decimal
+from decimal import ROUND_HALF_UP, Context, Decimal
 
 from ..frame import as_frame, kind_of
 
 _QUANT = {4: Decimal("0.0001")}
+_WIDE = Context(prec=340)
 
 
 def attributeType_segregation(idf):
@@ -87,7 +88,9 @@ def spark_round(x, scale=4):
     q = _QUANT.get(scale)
     if q is None:
         q = _QUANT[scale] = Decimal(1).scaleb(-scale)
-    return float(Decimal(repr(x)).quantize(q, rounding=ROUND_HALF_UP))
+    # Spark's BigDecimal has no digit limit: a variance of a bigint column (~1e37) has more digits than the default
+    # 28-digit context can quantize to `scale` places, so the context holds every digit a double can have
+    return float(Decimal(repr(x)).quantize(q, rounding=ROUND_HALF_UP, context=_WIDE))
 
 
 def spark_round_array(x, scale=4):

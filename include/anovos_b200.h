@@ -192,7 +192,11 @@ long long anv_gk_partition_sketch(const double* sorted_batches, long long n_valu
  * (-0.0 == 0.0, all NaNs equal).  Since the keys end up fully sorted, exact order statistics
  * are free: ranks [dev] n_cols * n_ranks 1-based ranks among the non-null values (0 = skip,
  * n_ranks may be 0) -> rank_values [dev] n_cols * n_ranks (the summary() percentiles of
- * stats_generator.py:488,813,908 without a separate selection pass). */
+ * stats_generator.py:488,813,908 without a separate selection pass).
+ * mode_value of an ANV_I64 column is NOT a double: its 8-byte slot holds the mode as an int64, bit for bit, and the
+ * caller reads it as int64_t (a double is exact only up to 2^53, and Spark returns the mode of a bigint column as a
+ * long).  The slot of an empty ANV_I64 column is unspecified (mode_rows 0 tells).  Every other dtype gets a double.
+ * rank_values stay doubles for every dtype, like Spark's summary() percentiles of a bigint column. */
 size_t anv_mode_distinct_workspace_bytes(int n_cols, int64_t n_rows, int key_bits);
 int anv_mode_distinct(const anv_column_t* cols, int n_cols, int64_t n_rows, int key_bits,
                       double* mode_value, int64_t* mode_rows, int64_t* n_distinct, const int64_t* ranks,

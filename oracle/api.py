@@ -508,8 +508,7 @@ def attribute_binning(table, list_of_cols="all", drop_cols=[], method_type="equa
     n_over = (len(cuts[0]) + 1) if cuts else bin_size            # :269 quirk (Appendix C #3)
     for c, cut in zip(cols, cuts):
         p = _profiles(table, [c])[c]
-        x = p.values.astype(np.float64)
-        ids = S.assign_bins(x, p.valid, cut, bin_size)
+        ids = S.assign_bins(p.values, p.valid, cut, bin_size)   # the column's own values: a bigint compares exactly
         ids[(ids == len(cut) + 1)] = n_over
         if bin_dtype == "numerical":
             arr = pa.array(ids, type=pa.int32(), mask=~p.valid)

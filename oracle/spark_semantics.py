@@ -114,7 +114,11 @@ def round_half_up(x, scale: int = 4):
     q = _Q.get(scale)
     if q is None:
         q = _Q[scale] = decimal.Decimal(1).scaleb(-scale)
-    return float(decimal.Decimal(repr(x)).quantize(q, rounding=decimal.ROUND_HALF_UP))
+    # BigDecimal has no digit limit: the context must hold all ~309 integer digits of a double and the scale
+    return float(decimal.Decimal(repr(x)).quantize(q, rounding=decimal.ROUND_HALF_UP, context=_WIDE))
+
+
+_WIDE = decimal.Context(prec=340)
 
 
 def java_double_to_string(x: float) -> str:

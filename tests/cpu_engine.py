@@ -49,13 +49,23 @@ def moments(fr, names):
     return out
 
 
+def _bin_ids(fr, model, i):
+    """Bin ids of column i of `model` (0 = null): from the exact int64 thresholds when the model has them
+    (bin 1 + #(thresholds < v), the kernels' compare), else from the float64 cutoffs."""
+    vals, valid = _values(fr, model.names[i])
+    ex = getattr(model, "exact", [None] * len(model.names))[i]
+    if ex is None:
+        return S.assign_bins(vals, valid, model.cutoffs[i], len(model.cutoffs[i]) + 1)
+    ids = 1 + np.searchsorted(np.array(ex, dtype=np.int64), vals.astype(np.int64), side="left")
+    return np.where(valid, ids, 0).astype(np.int32)
+
+
 def histogram(fr, model):
     if getattr(fr, "is_partitioned", False):
         return fr.histogram(model)
     h = np.zeros((len(model.names), model.max_bins + 1), np.uint64)
     for i, n in enumerate(model.names):
-        vals, valid = _values(fr, n)
-        ids = S.assign_bins(vals, valid, model.cutoffs[i], len(model.cutoffs[i]) + 1)
+        ids = _bin_ids(fr, model, i)
         h[i, :len(model.cutoffs[i]) + 2] = np.bincount(ids, minlength=len(model.cutoffs[i]) + 2)
     return h
 
@@ -147,16 +157,24 @@ def select_ranks(fr, names, ranks):
 
 
 def sort_mode_distinct(fr, names, ranks=None):
+    """Modes of bigint columns are exact Python ints (engine.sort_mode_distinct's contract), every other mode a float."""
     names = list(names)
     whole = _sorted_valid(fr, names)
     res = []
     for n in names:
-        x = whole[n] + 0.0
+        if fr.column(n).anv_dtype == _lib.ANV_I64:
+            if getattr(fr, "is_partitioned", False):
+                x = np.concatenate([_values(ch, n)[0][_values(ch, n)[1]] for ch in fr.chunks([n])] or [np.zeros(0, np.int64)])
+            else:
+                x = _values(fr, n)[0][_values(fr, n)[1]]
+            x = x.astype(np.int64)
+        else:
+            x = whole[n] + 0.0
         if x.size == 0:
             res.append((None, None, 0))
             continue
         u, k = np.unique(x, return_counts=True)
-        res.append((float(u[np.argmax(k)]), int(k.max()), int(u.size)))
+        res.append((u[np.argmax(k)].item(), int(k.max()), int(u.size)))
     if ranks is None:
         return res
     return res, select_ranks(fr, names, ranks)
@@ -177,8 +195,7 @@ def bin_assign(fr, model):
     import torch
     out = np.zeros((max(len(model.names), 1), fr.n_rows), np.int32)
     for i, n in enumerate(model.names):
-        vals, valid = _values(fr, n)
-        out[i] = S.assign_bins(vals, valid, model.cutoffs[i], len(model.cutoffs[i]) + 1)
+        out[i] = _bin_ids(fr, model, i)
     return torch.from_numpy(out)[:len(model.names)]
 
 

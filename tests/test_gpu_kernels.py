@@ -255,7 +255,7 @@ def test_mode_distinct_exact(n, sort_algo):
         u, k = np.unique(x, return_counts=True)
         assert nd == u.size, c                          # exact distinct
         assert rows == int(k.max()), c                  # exact mode_rows
-        assert mode == float(u[np.argmax(k)]), c        # smallest value among ties
+        assert mode == u[np.argmax(k)].item(), c        # smallest value among ties; an int64 mode compares exactly
 
 
 def test_hll_matches_oracle_registers(income):
