@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("ANOVOS_B200_LIB") or os.path.join(HERE, "libanovos_b200.so")
 
 ANV_F32, ANV_F64, ANV_I32, ANV_I64 = 0, 1, 2, 3
+MAX_LAUNCH_COLS = 65535   # ANV_MAX_LAUNCH_COLS of the header: columns per call of an entry point taking descriptors
 
 
 class AnvColumn(C.Structure):

@@ -129,7 +129,7 @@ extern "C" int anv_hll_registers(const anv_column_t* cols, int n_cols, int64_t n
                                  void* stream) {
   if (n_cols < 0 || n_rows < 0 || p < 4 || p > 18) { set_error("anv_hll_registers: bad arguments (4 <= p <= 18)"); return ANV_ERR_INVALID; }
   if (n_cols == 0) return ANV_OK;
-  if (n_cols > 65535) { set_error("n_cols > 65535"); return ANV_ERR_UNSUPPORTED; }
+  if (n_cols > ANV_MAX_LAUNCH_COLS) { set_error("n_cols > %d: split the frame into column blocks", ANV_MAX_LAUNCH_COLS); return ANV_ERR_UNSUPPORTED; }
   if (!cols || !regs) { set_error("anv_hll_registers: NULL argument"); return ANV_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   ANV_CUDA(cudaMemsetAsync(regs, 0, ((size_t)n_cols << p) * sizeof(uint32_t), st));

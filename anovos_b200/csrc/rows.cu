@@ -28,7 +28,8 @@ namespace anv {
 
 // ---- row null counts ------------------------------------------------------------------------------------------------
 
-constexpr int NC_PLANES = 17;                 // bit-sliced counters up to 2^17 - 1 >= 65535 columns
+constexpr int NC_PLANES = 17;                 // bit-sliced counters up to 2^17 - 1 columns
+constexpr int NC_MAX_COLS = (1 << NC_PLANES) - 1;   // one grid over the rows: the column count is bounded by the planes only
 constexpr int NC_SMEM_SLOTS = 6144;           // shared histogram (48 KB of uint64) for up to 6143 columns
 
 __global__ void __launch_bounds__(ANV_BLOCK) row_null_counts_kernel(const uint32_t* const* __restrict__ validity, int n_bm,
@@ -432,7 +433,7 @@ using namespace anv;
 extern "C" int anv_row_null_counts(const uint32_t* const* validity, int n_bitmaps, int n_cols, int64_t n_rows, int max_keep,
                                    uint64_t* counts, uint32_t* keep, void* stream) {
   if (n_bitmaps < 0 || n_cols < 0 || n_bitmaps > n_cols || n_rows < 0) { set_error("anv_row_null_counts: bad arguments"); return ANV_ERR_INVALID; }
-  if (n_cols > 65535) { set_error("n_cols > 65535"); return ANV_ERR_UNSUPPORTED; }
+  if (n_cols > NC_MAX_COLS) { set_error("anv_row_null_counts: n_cols > %d", NC_MAX_COLS); return ANV_ERR_UNSUPPORTED; }
   if (!counts || (n_bitmaps > 0 && !validity)) { set_error("anv_row_null_counts: NULL argument"); return ANV_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
   const int n_slots = n_cols + 1;
@@ -457,7 +458,7 @@ extern "C" size_t anv_row_distinct_workspace_bytes(int64_t n_rows) {
 extern "C" int anv_row_distinct(const anv_column_t* cols, int n_cols, int64_t n_rows, int hash_bits, int64_t* n_distinct,
                                 uint32_t* first, void* workspace, size_t workspace_bytes, void* stream) {
   if (n_cols < 0 || n_rows < 0 || hash_bits < 0 || hash_bits > 64) { set_error("anv_row_distinct: bad arguments"); return ANV_ERR_INVALID; }
-  if (n_cols > 65535) { set_error("n_cols > 65535"); return ANV_ERR_UNSUPPORTED; }
+  if (n_cols > ANV_MAX_LAUNCH_COLS) { set_error("anv_row_distinct: n_cols > %d is not supported", ANV_MAX_LAUNCH_COLS); return ANV_ERR_UNSUPPORTED; }
   if (n_rows >= ((int64_t)1 << 32)) { set_error("anv_row_distinct: n_rows >= 2^32 is not supported"); return ANV_ERR_UNSUPPORTED; }
   if (!n_distinct || !first || !workspace || (n_cols > 0 && !cols)) { set_error("anv_row_distinct: NULL argument"); return ANV_ERR_INVALID; }
   const RowLayout L(n_rows);

@@ -70,7 +70,7 @@ size_t hist_smem(int count_stride, int* path, int* thr_slots, bool codes) {
 
 int check_common(const void* cols, int n_cols, int64_t n_rows) {
   if (n_cols < 0 || n_rows < 0) { set_error("negative n_cols / n_rows"); return ANV_ERR_INVALID; }
-  if (n_cols > 65535) { set_error("n_cols > 65535: split the frame into column blocks"); return ANV_ERR_UNSUPPORTED; }
+  if (n_cols > ANV_MAX_LAUNCH_COLS) { set_error("n_cols > %d: split the frame into column blocks", ANV_MAX_LAUNCH_COLS); return ANV_ERR_UNSUPPORTED; }
   if (n_cols > 0 && !cols) { set_error("cols is NULL"); return ANV_ERR_INVALID; }
   return ANV_OK;
 }

@@ -369,7 +369,7 @@ int sel_check(const char* who, int n_cols, int n_ranks, int key_bits, const void
     set_error("%s: bad arguments (1 <= n_ranks <= %d, key_bits 32|64)", who, SEL_MAX_RANKS);
     return ANV_ERR_INVALID;
   }
-  if (n_cols > 65535) { set_error("n_cols > 65535"); return ANV_ERR_UNSUPPORTED; }
+  if (n_cols > ANV_MAX_LAUNCH_COLS) { set_error("n_cols > %d: split the frame into column blocks", ANV_MAX_LAUNCH_COLS); return ANV_ERR_UNSUPPORTED; }
   if (n_cols && !ws) { set_error("%s: NULL workspace", who); return ANV_ERR_INVALID; }
   if (n_cols && ws_bytes < anv_select_workspace_bytes(n_cols, n_ranks)) {
     set_error("%s: workspace too small", who);

@@ -2233,7 +2233,7 @@ extern "C" int anv_mode_distinct_hll(const anv_column_t* cols, int n_cols, int64
   if (n_cols < 0 || n_rows < 0 || (key_bits != 32 && key_bits != 64)) { set_error("anv_mode_distinct: bad arguments"); return ANV_ERR_INVALID; }
   if (hll_regs && (hll_p < 4 || hll_p > 12)) { set_error("anv_mode_distinct_hll: 4 <= hll_p <= 12"); return ANV_ERR_INVALID; }
   if (n_cols == 0) return ANV_OK;
-  if (n_cols > 65535) { set_error("n_cols > 65535"); return ANV_ERR_UNSUPPORTED; }
+  if (n_cols > ANV_MAX_LAUNCH_COLS) { set_error("n_cols > %d: split the frame into column blocks", ANV_MAX_LAUNCH_COLS); return ANV_ERR_UNSUPPORTED; }
   if (n_rows >= ((int64_t)1 << 32)) { set_error("anv_mode_distinct: n_rows >= 2^32 per call is not supported"); return ANV_ERR_UNSUPPORTED; }
   if (!cols || !mode_value || !mode_rows || !n_distinct || !workspace) { set_error("anv_mode_distinct: NULL argument"); return ANV_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
@@ -2261,7 +2261,7 @@ extern "C" int anv_mode_distinct_partition_hll(const anv_column_t* cols, int n_c
   if (n_cols < 0 || n_rows < 0) { set_error("anv_mode_distinct_partition: bad arguments"); return ANV_ERR_INVALID; }
   if (hll_regs && (hll_p < 4 || hll_p > 12)) { set_error("anv_mode_distinct_partition_hll: 4 <= hll_p <= 12"); return ANV_ERR_INVALID; }
   if (n_cols == 0) return ANV_OK;
-  if (n_cols > 65535) { set_error("n_cols > 65535"); return ANV_ERR_UNSUPPORTED; }
+  if (n_cols > ANV_MAX_LAUNCH_COLS) { set_error("n_cols > %d: split the frame into column blocks", ANV_MAX_LAUNCH_COLS); return ANV_ERR_UNSUPPORTED; }
   if (n_rows >= ((int64_t)1 << 32)) { set_error("anv_mode_distinct_partition: n_rows >= 2^32 per call is not supported"); return ANV_ERR_UNSUPPORTED; }
   if (!cols || !mode_value || !mode_rows || !n_distinct || !workspace) { set_error("anv_mode_distinct_partition: NULL argument"); return ANV_ERR_INVALID; }
   return run_partition_count(cols, n_cols, n_rows, mode_value, mode_rows, n_distinct, ranks, n_ranks, rank_values, hll_p, hll_regs,

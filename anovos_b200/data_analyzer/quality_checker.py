@@ -42,11 +42,8 @@ def _as_bool(v, what):
 
 
 def _unique(cols, drop):
-    out = []
-    for c in cols:
-        if c not in drop and c not in out:
-            out.append(c)
-    return out
+    drop = set(drop)
+    return [c for c in dict.fromkeys(cols) if c not in drop]     # first-seen order; sets keep wide frames linear
 
 
 def _read_stats(spec, columns):
@@ -69,7 +66,8 @@ def _row_cols(fr, list_of_cols, drop_cols):
         num, cat, _ = attributeType_segregation(fr)
         list_of_cols = num + cat
     cols = _unique(_names(list_of_cols), _names(drop_cols))
-    if any(c not in fr.columns for c in cols) or len(cols) == 0:
+    known = set(fr.columns)
+    if any(c not in known for c in cols) or len(cols) == 0:
         raise TypeError("Invalid input for Column(s)")
     other = [c for c in cols if fr.column(c).kind == "other"]
     if other:

@@ -5,6 +5,7 @@ current CUDA stream.  torch is plumbing only: device buffers and streams.
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import math
 
@@ -98,6 +99,27 @@ def _to_dev(arr: np.ndarray):
     return torch.from_numpy(np.ascontiguousarray(arr).view(np.uint8).reshape(-1)).cuda()
 
 
+def _in_column_blocks(call, n_cols):
+    """call(lo, hi) over consecutive column blocks [lo, hi) of at most _lib.MAX_LAUNCH_COLS columns, the most one launch
+    of a per-column pass takes, with the per-block results joined along the column axis: NumPy arrays and CUDA tensors
+    concatenated, lists chained, tuples joined element by element.  Up to that many columns it is call(0, n_cols) itself.
+    Every per-column result depends on its own column only, so the blocks give the results of one wide call."""
+    if n_cols <= _lib.MAX_LAUNCH_COLS:
+        return call(0, n_cols)
+    parts = [call(lo, min(lo + _lib.MAX_LAUNCH_COLS, n_cols)) for lo in range(0, n_cols, _lib.MAX_LAUNCH_COLS)]
+
+    def join(xs):
+        if isinstance(xs[0], list):
+            return [v for x in xs for v in x]
+        if isinstance(xs[0], tuple):
+            return tuple(join(list(t)) for t in zip(*xs))
+        if isinstance(xs[0], np.ndarray):
+            return np.concatenate(xs)
+        import torch
+        return torch.cat(xs)
+    return join(parts)
+
+
 # ---- K1 ---------------------------------------------------------------------------------
 
 def moments(frame: ColumnFrame, names):
@@ -108,6 +130,8 @@ def moments(frame: ColumnFrame, names):
     torch = _lib.require_cuda()
     L = _lib.lib()
     names = list(names)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: moments(frame, names[lo:hi]), len(names))
     if not names:
         return np.zeros(0, dtype=_MOM_DT)
     desc, keep = frame.descriptors(names)
@@ -223,6 +247,15 @@ class BinModel:
         self.cuts_host = np.concatenate(raws) if raws else np.zeros(1, np.uint64)
         self._dev = None
 
+    def block(self, lo, hi):
+        """The model of columns [lo, hi): their specs with the same thresholds (cut_offset indexes the whole `cuts`) and
+        the same max_bins, so the count strides of the blocks agree."""
+        sub = copy.copy(self)
+        sub.names, sub.cutoffs, sub.exact = self.names[lo:hi], self.cutoffs[lo:hi], self.exact[lo:hi]
+        sub.specs_host = self.specs_host[lo:hi]
+        sub._dev = None
+        return sub
+
     def device(self):
         if self._dev is None:
             self._dev = (_to_dev(self.specs_host), _to_dev(self.cuts_host if self.cuts_host.size else np.zeros(1, np.uint64)))
@@ -239,6 +272,8 @@ def histogram(frame: ColumnFrame, model: BinModel):
     _lib.require_cuda()
     L = _lib.lib()
     n = len(model.names)
+    if n > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: histogram(frame, model.block(lo, hi)), n)
     stride = model.max_bins + 1
     if n == 0:
         return np.zeros((0, stride), np.uint64)
@@ -259,6 +294,8 @@ def moments_histogram(frame: ColumnFrame, model: BinModel):
     _lib.require_cuda()
     L = _lib.lib()
     n = len(model.names)
+    if n > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: moments_histogram(frame, model.block(lo, hi)), n)
     stride = model.max_bins + 1
     if n == 0:
         return np.zeros(0, dtype=_MOM_DT), np.zeros((0, stride), np.uint64)
@@ -284,6 +321,8 @@ def bin_assign(frame: ColumnFrame, model: BinModel):
     torch = _lib.require_cuda()
     L = _lib.lib()
     n = len(model.names)
+    if n > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: bin_assign(frame, model.block(lo, hi)), n)
     stride = (frame.n_rows + 3) // 4 * 4
     out = torch.empty((max(n, 1), max(stride, 4)), dtype=torch.int32, device="cuda")
     if n == 0 or frame.n_rows == 0:
@@ -305,6 +344,9 @@ def code_counts(frame: ColumnFrame, names):
     global launch_count
     _lib.require_cuda()
     L = _lib.lib()
+    names = list(names)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: code_counts(frame, names[lo:hi]), len(names))
     out = {}
     groups = {}
     for nme in names:
@@ -384,6 +426,8 @@ def select_ranks(frame: ColumnFrame, names, ranks):
     L = _lib.lib()
     names = list(names)
     ranks = np.ascontiguousarray(ranks, dtype=np.int64).reshape(len(names), -1)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: select_ranks(frame, names[lo:hi], ranks[lo:hi]), len(names))
     out = np.full(ranks.shape, np.nan, np.float64)
     if not names or ranks.shape[1] == 0:
         return out
@@ -416,14 +460,15 @@ FUSED_HLL = True                  # sort_mode_distinct(..., hll_p=p) also return
 
 
 def _mode_distinct_batch_size(frame, n_cols, per_col_bytes):
-    """Columns per sort launch: the scratch of a batch stays under SORT_WORKSPACE_BUDGET and under 80 % of the memory that is
-    not held by live tensors (torch's allocator statistics: no driver call - cudaMemGetInfo costs ~7 ms)."""
+    """Columns per sort launch: at most _lib.MAX_LAUNCH_COLS, and the scratch of a batch stays under SORT_WORKSPACE_BUDGET and
+    under 80 % of the memory that is not held by live tensors (torch's allocator statistics: no driver call - cudaMemGetInfo
+    costs ~7 ms)."""
     torch = _lib.require_cuda()
     budget = SORT_WORKSPACE_BUDGET
     if per_col_bytes * n_cols > (2 << 30):
         total = torch.cuda.get_device_properties(torch.cuda.current_device()).total_memory
         budget = min(budget, int((total - torch.cuda.memory_allocated()) * 0.8))
-    return max(1, min(n_cols, budget // max(per_col_bytes, 1)))
+    return max(1, min(n_cols, _lib.MAX_LAUNCH_COLS, budget // max(per_col_bytes, 1)))
 
 
 def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
@@ -562,6 +607,9 @@ def row_distinct(frame: ColumnFrame, names, hash_bits=0):
     names = list(names)
     if frame.n_rows >= (1 << 32):
         raise _lib.AnvError("row_distinct: frames of 2^32 rows or more are not supported")
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        raise NotImplementedError("distinct rows over more than %d columns are not supported: rows are compared whole, so "
+                                  "the columns cannot be split into blocks" % _lib.MAX_LAUNCH_COLS)
     desc, keep = frame.descriptors(names) if names else (_dev_bytes(16), None)
     ws_bytes = L.anv_row_distinct_workspace_bytes(frame.n_rows)
     ws = _dev_bytes(ws_bytes)
@@ -667,6 +715,8 @@ def hll_registers(frame: ColumnFrame, names, p: int):
     _lib.require_cuda()
     L = _lib.lib()
     names = list(names)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: hll_registers(frame, names[lo:hi], p), len(names))
     m = 1 << p
     desc, keep = frame.descriptors(names)
     regs = _dev_bytes(len(names) * m * 4)

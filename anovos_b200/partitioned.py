@@ -328,6 +328,8 @@ class PartitionedFrame:
         L = _lib.lib()
         names = list(names)
         ranks = np.ascontiguousarray(ranks, dtype=np.int64).reshape(len(names), -1)
+        if len(names) > _lib.MAX_LAUNCH_COLS:
+            return engine._in_column_blocks(lambda lo, hi: self.select_ranks(names[lo:hi], ranks[lo:hi]), len(names))
         out = np.full(ranks.shape, np.nan, np.float64)
         if not names or ranks.shape[1] == 0:
             return out

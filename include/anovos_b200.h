@@ -31,6 +31,11 @@ extern "C" {
 
 #define ANV_VERSION 100 /* 0.1.0 */
 
+/* Most column passes launch one grid row per column (gridDim.y <= 65535): the entry points that take anv_column_t
+ * descriptors reject more columns per call with ANV_ERR_UNSUPPORTED, and a caller splits a wider frame into column
+ * blocks of at most this many (every per-column result is independent of the other columns of the call). */
+#define ANV_MAX_LAUNCH_COLS 65535
+
 typedef enum {
   ANV_OK = 0,
   ANV_ERR_INVALID = -1,   /* bad argument (null pointer, misaligned column, bad dtype ...) */
@@ -232,7 +237,8 @@ int anv_mode_distinct_partition(const anv_column_t* cols, int n_cols, int64_t n_
  *      then groupBy(null_cols_count).count()).  validity [dev] n_bitmaps device pointers to the Arrow bitmaps of the
  *      columns that HAVE one (a column without a bitmap adds nothing; n_cols counts every column and sizes `counts`).
  *      NaN is not null.  counts [dev] n_cols + 1 uint64: slot k = rows with k null columns (zeroed by the library).
- *      keep [dev] ceil(n_rows/32) bitmap words or NULL: bit set where the row's count <= max_keep (max_keep < 0: none). */
+ *      keep [dev] ceil(n_rows/32) bitmap words or NULL: bit set where the row's count <= max_keep (max_keep < 0: none).
+ *      n_cols <= 131071 (17 bit planes per row count; the grid runs over rows only, so ANV_MAX_LAUNCH_COLS does not apply). */
 int anv_row_null_counts(const uint32_t* const* validity, int n_bitmaps, int n_cols, int64_t n_rows, int max_keep,
                         uint64_t* counts, uint32_t* keep, void* stream);
 
@@ -243,7 +249,8 @@ int anv_row_null_counts(const uint32_t* const* validity, int n_bitmaps, int n_co
  *      compared with its group's first row, so the result never depends on the hash being unique.
  *      hash_bits caps the hash bits kept in the sort key (0 = all that fit above the row index; 1-8 send nearly every
  *      row through the comparison path, for testing).  n_distinct [dev] 1 int64; first [dev] ceil(n_rows/32) bitmap
- *      words, bit set on the first occurrence of every distinct row (row order).  n_rows >= 2^32: ANV_ERR_UNSUPPORTED. */
+ *      words, bit set on the first occurrence of every distinct row (row order).  n_rows >= 2^32 or
+ *      n_cols > ANV_MAX_LAUNCH_COLS: ANV_ERR_UNSUPPORTED (rows are compared whole, so a caller cannot split the columns). */
 size_t anv_row_distinct_workspace_bytes(int64_t n_rows);
 int anv_row_distinct(const anv_column_t* cols, int n_cols, int64_t n_rows, int hash_bits, int64_t* n_distinct,
                      uint32_t* first, void* workspace, size_t workspace_bytes, void* stream);

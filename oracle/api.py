@@ -61,18 +61,15 @@ def _split(x):
 
 
 def _dedupe(cols, drop):
-    out = []
-    for c in cols:
-        if c not in drop and c not in out:
-            out.append(c)
-    return out  # reference: list(set(...)) - order arbitrary, we keep input order
+    drop = set(drop)
+    return [c for c in dict.fromkeys(cols) if c not in drop]  # reference: list(set(...)) - order arbitrary, we keep input order
 
 
 def _resolve(table, list_of_cols, drop_cols, default, universe=None, allow_empty=False):
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = default
     cols = _dedupe(_split(list_of_cols), _split(drop_cols))
-    universe = table.column_names if universe is None else universe
+    universe = set(table.column_names if universe is None else universe)
     if any(c not in universe for c in cols) or (len(cols) == 0 and not allow_empty):
         raise TypeError("Invalid input for Column(s)")
     return cols
@@ -182,7 +179,8 @@ class ColumnProfile:
         if self.sdtype == "string":
             u, c = np.unique(self.nn.astype(str), return_counts=True)
         else:
-            u, c = np.unique(self.nn, return_counts=True)
+            # Spark 3 groups -0.0 with 0.0 under the key 0.0 (NormalizeFloatingNumbers)
+            u, c = np.unique(self.nn + 0.0 if self.nn.dtype.kind == "f" else self.nn, return_counts=True)
         i = int(np.argmax(c))
         return u[i], int(c[i])
 

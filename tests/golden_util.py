@@ -62,7 +62,7 @@ def assert_frames_match(got, exp, flip=1.0001e-4, rel=1e-9):
                     band = flip * (1.0 + 2.0 * abs(float(e)) ** 0.5)
                 elif c == "cov":
                     band = flip * (1.0 + abs(float(e)))
-                ok = abs(float(g) - float(e)) <= band + rel * abs(float(e))
+                ok = float(g) == float(e) or abs(float(g) - float(e)) <= band + rel * abs(float(e))   # equal infinities too
             if not ok:
                 bad.append((a, c, g, e))
     assert not bad, bad[:20]

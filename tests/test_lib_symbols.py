@@ -26,6 +26,12 @@ def test_library_builds_and_exports_every_declared_symbol():
     assert _lib.lib().anv_version() == 100
 
 
+def test_column_block_limit_matches_header():
+    from anovos_b200 import _lib
+    h = open(os.path.join(ROOT, "include", "anovos_b200.h")).read()
+    assert int(re.search(r"#define ANV_MAX_LAUNCH_COLS (\d+)", h).group(1)) == _lib.MAX_LAUNCH_COLS == 65535
+
+
 def test_struct_layouts_match_header():
     from anovos_b200 import _lib, engine
     assert ctypes.sizeof(_lib.AnvColumn) == 24 and ctypes.sizeof(_lib.AnvMoments) == 64
