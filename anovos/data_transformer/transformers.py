@@ -1,1 +1,1 @@
-from anovos_b200.data_transformer.transformers import attribute_binning  # noqa: F401
+from anovos_b200.data_transformer.transformers import attribute_binning, imputation_MMM  # noqa: F401

@@ -35,6 +35,13 @@ class AnvDrift(C.Structure):
                 ("n_rows", C.c_int32), ("reserved", C.c_int32)]
 
 
+class AnvImputeSpec(C.Structure):
+    _fields_ = [("out_dtype", C.c_int32), ("flags", C.c_int32), ("fill", C.c_uint64)]
+
+
+IMPUTE_NAN_MISSING, IMPUTE_ROUND_DOUBLE = 1, 2   # ANV_IMPUTE_* flags of the header
+
+
 class AnvError(RuntimeError):
     pass
 
@@ -73,6 +80,8 @@ _SIGNATURES = {
     "anv_row_null_counts": (C.c_int, [_P, _I, _I, _L, _I, _P, _P, _P]),
     "anv_row_distinct_workspace_bytes": (_SZ, [_L]),
     "anv_row_distinct": (C.c_int, [_P, _I, _L, _I, _P, _P, _P, _SZ, _P]),
+    "anv_impute_fill": (C.c_int, [_P, _P, _P, _I, _L, _P]),
+    "anv_valid_not_nan": (C.c_int, [_P, _I, _L, _P, _P, _P]),
     "anv_spark_hash_seed": (C.c_uint64, [_L]),
     "anv_spark_sample_mask": (C.c_int, [_L, _L, _P, _P, _I, _P, _P]),
     "anv_synth_f32": (C.c_int, [_P, _P, _L, C.c_uint64, C.c_uint32, _I, C.c_float, C.c_float, C.c_float, _P]),

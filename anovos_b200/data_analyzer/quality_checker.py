@@ -228,6 +228,21 @@ def nullColumns_detection(spark, idf, list_of_cols="missing", drop_cols=[], trea
             if print_impact:
                 print("Before Count: " + str(fr.count()))
                 print("After Count: " + str(odf.count()))
+        elif treatment_method == "MMM":
+            # reference :491-519: drop columns with fewer than 2 distinct values, apply the threshold, impute
+            from ..data_transformer.transformers import imputation_MMM
+            from .stats_generator import uniqueCount_computation
+            if stats_unique == {}:
+                uq = uniqueCount_computation(spark, fr, cols).toPandas()
+            else:
+                uq = _read_stats(stats_unique, ["attribute", "unique_values"])
+            remove = set(uq.loc[uq["unique_values"] < 2, "attribute"].tolist())
+            sub = [c for c in cols if c not in remove]
+            if threshold:
+                sub = [c for c in threshold_cols if c not in remove]
+            odf = imputation_MMM(spark, fr, sub, **treatment_configs, stats_missing=stats_missing, stats_mode=stats_mode,
+                                 print_impact=print_impact)
+            return odf, ResultFrame(stats)        # the reference prints imputation_MMM's table only
         else:
             raise NotImplementedError("treatment_method=%r (imputation) is outside the GPU hot-path build" % treatment_method)
     out = ResultFrame(stats)

@@ -752,3 +752,98 @@ def hll_estimates(frame: ColumnFrame, names, p: int):
         for n, r in zip(cat, hll_estimates_from_register_rows(R, p)):
             out[n] = r
     return [out[n] for n in names]
+
+
+# ---- imputation --------------------------------------------------------------------------------
+
+_IMPUTE_SPEC_DT = np.dtype([("out_dtype", "<i4"), ("flags", "<i4"), ("fill", "<u8")])
+_FILL_PAIRS = {(_lib.ANV_F32, _lib.ANV_F32), (_lib.ANV_F64, _lib.ANV_F64), (_lib.ANV_I32, _lib.ANV_I32),
+               (_lib.ANV_I64, _lib.ANV_I64), (_lib.ANV_I32, _lib.ANV_F64), (_lib.ANV_I64, _lib.ANV_F64)}
+_TORCH_OF_ANV = {_lib.ANV_F32: "float32", _lib.ANV_F64: "float64", _lib.ANV_I32: "int32", _lib.ANV_I64: "int64"}
+
+
+def java_cast(x, anv_dtype):
+    """A double cast to the column type the way the JVM casts it (Spark's `cast` of a double): (float) rounds to nearest,
+    d2i / d2l truncate toward zero, saturate at the type's range and map NaN to 0.  -> Python float or int."""
+    x = float(x)
+    if anv_dtype == _lib.ANV_F64:
+        return x
+    if anv_dtype == _lib.ANV_F32:
+        with np.errstate(over="ignore"):
+            return float(np.float32(x))
+    lo, hi = (-(1 << 31), (1 << 31) - 1) if anv_dtype == _lib.ANV_I32 else (I64_MIN, I64_MAX)
+    if x != x:
+        return 0
+    if x >= hi:            # hi + 1 is a power of two: every double at or above hi saturates
+        return hi
+    if x <= lo:
+        return lo
+    return int(x)          # truncation toward zero; exact, |x| < 2^63
+
+
+def fill_bits(value, anv_dtype) -> int:
+    """The fill value's bits in an output column of `anv_dtype` (the `fill` slot of anv_impute_spec_t): value must be
+    representable (java_cast it first)."""
+    if anv_dtype == _lib.ANV_F32:
+        return int(np.array([value], np.float32).view(np.uint32)[0])
+    if anv_dtype == _lib.ANV_F64:
+        return int(np.array([value], np.float64).view(np.uint64)[0])
+    if anv_dtype == _lib.ANV_I32:
+        return int(np.array([value], np.int32).view(np.uint32)[0])
+    return int(np.array([value], np.int64).view(np.uint64)[0])
+
+
+def impute_fill(frame: ColumnFrame, names, out_dtypes, flags, fills):
+    """-> list of dense CUDA tensors [n_rows] (one per name, no nulls): anv_impute_fill with per-column output dtype, flags
+    (_lib.IMPUTE_*) and fill bits (fill_bits).  One streaming pass over the columns."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names = list(names)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: impute_fill(frame, names[lo:hi], out_dtypes[lo:hi], flags[lo:hi], fills[lo:hi]),
+                                 len(names))
+    if not names:
+        return []
+    specs = np.zeros(len(names), _IMPUTE_SPEC_DT)
+    outs, ptrs = [], np.zeros(len(names), np.uint64)
+    padded = (frame.n_rows + 3) // 4 * 4
+    for i, (n, od, fl, fv) in enumerate(zip(names, out_dtypes, flags, fills)):
+        ind = frame.column(n).anv_dtype
+        if (ind, od) not in _FILL_PAIRS or (fl & _lib.IMPUTE_NAN_MISSING and ind not in (_lib.ANV_F32, _lib.ANV_F64)):
+            raise ValueError("impute_fill: column %r: no fill from dtype %d to %d with flags %d" % (n, ind, od, fl))
+        specs[i] = (od, fl, fv)
+        t = torch.empty(max(padded, 4), dtype=getattr(torch, _TORCH_OF_ANV[od]), device="cuda")
+        outs.append(t)
+        ptrs[i] = t.data_ptr()
+    if frame.n_rows:
+        desc, keep = frame.descriptors(names)
+        dspecs, dptrs = _to_dev(specs), _to_dev(ptrs)
+        nbytes = input_bytes(frame, names)
+        if timer is not None:
+            nbytes += sum(frame.n_rows * t.element_size() for t in outs)
+        _call(L.anv_impute_fill, "anv_impute_fill", desc.data_ptr(), dspecs.data_ptr(), dptrs.data_ptr(), len(names),
+              frame.n_rows, _stream(), nbytes=nbytes)
+        launch_count += 1
+    return [t[:frame.n_rows] for t in outs]
+
+
+def valid_not_nan(frame: ColumnFrame, names):
+    """-> (int32 CUDA tensor [n_cols, ceil(n_rows/32)] of "non-null and not NaN" bitmap words, int64 ndarray of NaN counts
+    per column).  The Imputer's mean and median are the moments / selection of a view of the column with this bitmap."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names = list(names)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: valid_not_nan(frame, names[lo:hi]), len(names))
+    n_words = (frame.n_rows + 31) // 32
+    words = torch.zeros((max(len(names), 1), max(n_words, 1)), dtype=torch.int32, device="cuda")
+    if not names:
+        return words[:0, :n_words], np.zeros(0, np.int64)
+    desc, keep = frame.descriptors(names)
+    n_nan = _dev_bytes(len(names) * 8)
+    _call(L.anv_valid_not_nan, "anv_valid_not_nan", desc.data_ptr(), len(names), frame.n_rows, words.data_ptr(),
+          n_nan.data_ptr(), _stream(), nbytes=input_bytes(frame, names))
+    launch_count += 1
+    return words[:, :n_words], _host(n_nan).view(np.int64)[:len(names)].copy()

@@ -255,6 +255,32 @@ size_t anv_row_distinct_workspace_bytes(int64_t n_rows);
 int anv_row_distinct(const anv_column_t* cols, int n_cols, int64_t n_rows, int hash_bits, int64_t* n_distinct,
                      uint32_t* first, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- mean / median / mode imputation (imputation_MMM, data_transformer/transformers.py:1369-1676; the MMM treatment of
+ *      nullColumns_detection, data_analyzer/quality_checker.py:491-519).
+ * anv_impute_fill: one streaming pass per column writes a DENSE output column (no bitmap) of spec.out_dtype:
+ *   out[r] = (row r non-null && !(NAN_MISSING && isnan(x[r]))) ? convert(x[r]) : fill.
+ * (input dtype -> out_dtype) pairs: F32->F32, F64->F64, I32->I32 (numbers or dictionary codes), I64->I64, I32->F64 and
+ * I64->F64 (convert = (double)x); other pairs leave the output unwritten.  ANV_IMPUTE_NAN_MISSING (F32 / F64 inputs): NaN
+ * counts as missing, as in Spark's Imputer.  ANV_IMPUTE_ROUND_DOUBLE (I64 -> I64): convert = (long)(double)x, the round trip
+ * of Spark's recast to double and back (saturating like Java's d2l; for I32 the identity).  `fill` holds the fill value's
+ * bits in the output type (low 4 bytes for 4-byte types): the caller converts the surrogate.
+ * specs [dev] n_cols; out_ptrs [dev] n_cols device pointers, each 16-byte aligned with room for n_rows rounded up to a
+ * multiple of 4 elements. */
+#define ANV_IMPUTE_NAN_MISSING 1
+#define ANV_IMPUTE_ROUND_DOUBLE 2
+typedef struct {
+  int32_t out_dtype; /* anv_dtype of the output column */
+  int32_t flags;     /* ANV_IMPUTE_* */
+  uint64_t fill;     /* fill value bits in out_dtype */
+} anv_impute_spec_t;
+int anv_impute_fill(const anv_column_t* cols, const anv_impute_spec_t* specs, void* const* out_ptrs, int n_cols, int64_t n_rows,
+                    void* stream);
+/* The Imputer's statistics skip NaN as well as null: for every column, out_validity [dev] n_cols * ceil(n_rows/32) words
+ * (column c at out_validity + c * ceil(n_rows/32)) gets bit r set where row r is non-null and not NaN (bits past n_rows are
+ * 0), and n_nan [dev] n_cols int64 the number of non-null NaN rows (zeroed by the library).  Integer columns: the validity. */
+int anv_valid_not_nan(const anv_column_t* cols, int n_cols, int64_t n_rows, uint32_t* out_validity, int64_t* n_nan,
+                      void* stream);
+
 /* ---- Spark's Bernoulli row sampler (the DEFAULT path of drift_detector.statistics: use_sampling=True ->
  *      data_sampling.py:122-149 `idf.sample(False, fraction, seed)` / `stat.sampleBy("merge", fractions, seed)`,
  *      drift_detector.py:187-211).  One partition per call: Spark seeds XORShiftRandom with seed + partitionIndex,
