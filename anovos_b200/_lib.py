@@ -42,6 +42,15 @@ class AnvImputeSpec(C.Structure):
 IMPUTE_NAN_MISSING, IMPUTE_ROUND_DOUBLE = 1, 2   # ANV_IMPUTE_* flags of the header
 
 
+class AnvScaleSpec(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("out_dtype", C.c_int32), ("flags", C.c_int32), ("reserved", C.c_int32),
+                ("a", C.c_double), ("b", C.c_double), ("c", C.c_double)]
+
+
+SCALE_DIV, SCALE_AFFINE, SCALE_CONST = 0, 1, 2   # ANV_SCALE_* modes of the header
+SCALE_NAN_TO_NULL = 1                            # ANV_SCALE_NAN_TO_NULL
+
+
 class AnvError(RuntimeError):
     pass
 
@@ -82,6 +91,7 @@ _SIGNATURES = {
     "anv_row_distinct": (C.c_int, [_P, _I, _L, _I, _P, _P, _P, _SZ, _P]),
     "anv_impute_fill": (C.c_int, [_P, _P, _P, _I, _L, _P]),
     "anv_valid_not_nan": (C.c_int, [_P, _I, _L, _P, _P, _P]),
+    "anv_scale_columns": (C.c_int, [_P, _P, _P, _P, _P, _I, _L, _P]),
     "anv_spark_hash_seed": (C.c_uint64, [_L]),
     "anv_spark_sample_mask": (C.c_int, [_L, _L, _P, _P, _I, _P, _P]),
     "anv_synth_f32": (C.c_int, [_P, _P, _L, C.c_uint64, C.c_uint32, _I, C.c_float, C.c_float, C.c_float, _P]),

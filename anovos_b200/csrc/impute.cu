@@ -2,65 +2,16 @@
 // 1369-1676): the fill pass that writes the imputed columns, and the "non-null and not NaN" bitmap the Imputer's
 // statistics are taken over.
 //
-// Both passes stream each column once.  Grid (row tiles, columns); a warp covers 128 consecutive rows per step, four
-// per lane, so every lane moves its values with 128-bit loads and stores (two for 8-byte types).  The validity word of
-// 32 rows is loaded once, by one of the first four lanes, and handed to the eight lanes that cover its rows by a shuffle.
+// Both passes stream each column once.  Grid (row tiles, columns), four rows per lane with 128-bit loads and stores
+// (quad.cuh).
 //
 // Fill: out = (valid && !(nan_missing && isnan(x))) ? convert(x) : fill, dense, with no bitmap.  convert is the
 // identity, int -> double (numeric mode imputation keeps numbers in the recast type) or, for bigint under mean / median,
 // the round trip (long)(double)x of Spark's recast (cvt saturates like Java's d2l: 2^63-1 comes back as 2^63-1).  The
 // fill value arrives already converted to the output type: the kernel does no per-column double work.
-#include "common.cuh"
+#include "quad.cuh"
 
 namespace anv {
-
-constexpr int IMP_ROWS_PER_LANE = 4;
-constexpr int IMP_ROWS_PER_WARP = 32 * IMP_ROWS_PER_LANE;
-constexpr int IMP_ROWS_PER_CTA = ANV_BLOCK * IMP_ROWS_PER_LANE;
-
-// Four consecutive values from row r (r % 4 == 0) as 128-bit loads; a quad that crosses n_rows reads its live rows only.
-template <typename T> __device__ __forceinline__ void load_quad(const T* __restrict__ p, int64_t r, int64_t n_rows, T (&e)[4]) {
-  if (r + 4 <= n_rows) {
-    if constexpr (sizeof(T) == 4) {
-      unpack<T>(ldg_stream(p + r), e);
-    } else {
-      T a[2], b[2];
-      unpack<T>(ldg_stream(p + r), a);
-      unpack<T>(ldg_stream(p + r + 2), b);
-      e[0] = a[0]; e[1] = a[1]; e[2] = b[0]; e[3] = b[1];
-    }
-  } else {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) e[k] = (r + k < n_rows) ? p[r + k] : T(0);
-  }
-}
-
-// Four values to row r of an output padded to a multiple of 4 rows: always whole 128-bit stores.
-template <typename U> __device__ __forceinline__ void store_quad(U* __restrict__ p, int64_t r, const U (&e)[4]) {
-  if constexpr (sizeof(U) == 4) {
-    uint4 q;
-    q.x = reinterpret_cast<const uint32_t&>(e[0]); q.y = reinterpret_cast<const uint32_t&>(e[1]);
-    q.z = reinterpret_cast<const uint32_t&>(e[2]); q.w = reinterpret_cast<const uint32_t&>(e[3]);
-    __stcs(reinterpret_cast<uint4*>(p + r), q);
-  } else {
-    ulonglong2 a, b;
-    a.x = reinterpret_cast<const unsigned long long&>(e[0]); a.y = reinterpret_cast<const unsigned long long&>(e[1]);
-    b.x = reinterpret_cast<const unsigned long long&>(e[2]); b.y = reinterpret_cast<const unsigned long long&>(e[3]);
-    __stcs(reinterpret_cast<ulonglong2*>(p + r), a);
-    __stcs(reinterpret_cast<ulonglong2*>(p + r + 2), b);
-  }
-}
-
-// The 4 validity bits of the lane's quad: the warp's 128 rows span 4 bitmap words, loaded by lanes 0-3 and shuffled to
-// the 8 lanes each word covers.  NULL bitmap: every row valid.  Called by the whole warp (r0 is warp-uniform).
-__device__ __forceinline__ uint32_t quad_valid_bits(const uint32_t* __restrict__ validity, int64_t r0, int64_t n_rows, int lane) {
-  if (!validity) return 0xFu;
-  const int64_t w = r0 / 32 + lane;
-  const int64_t n_words = (n_rows + 31) / 32;
-  uint32_t word = (lane < 4 && w < n_words) ? __ldg(validity + w) : 0u;
-  word = __shfl_sync(ANV_FULL, word, lane >> 3);
-  return (word >> (4 * (lane & 7))) & 0xFu;
-}
 
 template <typename T, typename U, bool ROUND> __device__ __forceinline__ U convert(T x) {
   if constexpr (ROUND) return (U)(double)x;                  // bigint under mean / median: Spark's recast round trip
@@ -71,10 +22,10 @@ template <typename T, typename U, bool ROUND>
 __device__ __forceinline__ void fill_column(const T* __restrict__ src, const uint32_t* __restrict__ validity, U* __restrict__ dst,
                                             U fill, bool nan_missing, int64_t n_rows) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t step = (int64_t)gridDim.x * IMP_ROWS_PER_CTA;
-  for (int64_t r0 = (int64_t)blockIdx.x * IMP_ROWS_PER_CTA + (int64_t)warp * IMP_ROWS_PER_WARP; r0 < n_rows; r0 += step) {
+  const int64_t step = (int64_t)gridDim.x * QUAD_ROWS_PER_CTA;
+  for (int64_t r0 = (int64_t)blockIdx.x * QUAD_ROWS_PER_CTA + (int64_t)warp * QUAD_ROWS_PER_WARP; r0 < n_rows; r0 += step) {
     const uint32_t vb = quad_valid_bits(validity, r0, n_rows, lane);
-    const int64_t r = r0 + lane * IMP_ROWS_PER_LANE;
+    const int64_t r = r0 + lane * QUAD_ROWS_PER_LANE;
     if (r >= n_rows) continue;
     T e[4];
     load_quad<T>(src, r, n_rows, e);
@@ -137,11 +88,11 @@ __device__ __forceinline__ void valid_not_nan_column(const T* __restrict__ src, 
                                                      uint32_t* __restrict__ out, unsigned long long* __restrict__ n_nan,
                                                      int64_t n_rows) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t step = (int64_t)gridDim.x * IMP_ROWS_PER_CTA;
+  const int64_t step = (int64_t)gridDim.x * QUAD_ROWS_PER_CTA;
   unsigned long long nan_count = 0;
-  for (int64_t r0 = (int64_t)blockIdx.x * IMP_ROWS_PER_CTA + (int64_t)warp * IMP_ROWS_PER_WARP; r0 < n_rows; r0 += step) {
+  for (int64_t r0 = (int64_t)blockIdx.x * QUAD_ROWS_PER_CTA + (int64_t)warp * QUAD_ROWS_PER_WARP; r0 < n_rows; r0 += step) {
     const uint32_t vb = quad_valid_bits(validity, r0, n_rows, lane);
-    const int64_t r = r0 + lane * IMP_ROWS_PER_LANE;
+    const int64_t r = r0 + lane * QUAD_ROWS_PER_LANE;
     uint32_t keep = 0, nan = 0;
     if (r < n_rows) {
       T e[4];
@@ -182,17 +133,6 @@ __global__ void __launch_bounds__(ANV_BLOCK) valid_not_nan_kernel(const anv_colu
   }
 }
 
-// Row tiles per column: enough CTAs for ~16 per SM across the launch, never more than the rows need.
-static unsigned impute_grid_x(int64_t n_rows, int n_cols) {
-  int sms = 132, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int64_t need = (n_rows + IMP_ROWS_PER_CTA - 1) / IMP_ROWS_PER_CTA;
-  int64_t want = ((int64_t)sms * 16 + n_cols - 1) / n_cols;
-  if (want < 1) want = 1;
-  return (unsigned)(need < want ? need : want);
-}
-
 int check_common(const void* cols, int n_cols, int64_t n_rows);
 
 }  // namespace anv
@@ -205,7 +145,7 @@ extern "C" int anv_impute_fill(const anv_column_t* cols, const anv_impute_spec_t
   if (n_cols == 0 || n_rows == 0) return ANV_OK;
   if (!specs || !out_ptrs) { set_error("anv_impute_fill: specs / out_ptrs is NULL"); return ANV_ERR_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid(impute_grid_x(n_rows, n_cols), (unsigned)n_cols);
+  dim3 grid(quad_grid_x(n_rows, n_cols), (unsigned)n_cols);
   impute_fill_kernel<<<grid, ANV_BLOCK, 0, st>>>(cols, specs, out_ptrs, n_rows);
   ANV_CUDA(cudaGetLastError());
   return ANV_OK;
@@ -219,7 +159,7 @@ extern "C" int anv_valid_not_nan(const anv_column_t* cols, int n_cols, int64_t n
   cudaStream_t st = (cudaStream_t)stream;
   ANV_CUDA(cudaMemsetAsync(n_nan, 0, (size_t)n_cols * sizeof(int64_t), st));
   if (n_rows == 0) return ANV_OK;
-  dim3 grid(impute_grid_x(n_rows, n_cols), (unsigned)n_cols);
+  dim3 grid(quad_grid_x(n_rows, n_cols), (unsigned)n_cols);
   valid_not_nan_kernel<<<grid, ANV_BLOCK, 0, st>>>(cols, n_rows, out_validity, reinterpret_cast<unsigned long long*>(n_nan));
   ANV_CUDA(cudaGetLastError());
   return ANV_OK;

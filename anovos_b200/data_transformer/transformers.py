@@ -1,6 +1,6 @@
 """CUDA implementation of `anovos.data_transformer.transformers.attribute_binning`
-(reference /root/reference/src/main/anovos/data_transformer/transformers.py:87-291) and `imputation_MMM` (:1369-1676,
-at the end of this module).
+(reference /root/reference/src/main/anovos/data_transformer/transformers.py:87-291), `imputation_MMM` (:1369-1676) and
+the scalers `z_standardization`, `IQR_standardization` and `normalization` (:965-1366, at the end of this module).
 
 The reference computes the cutoffs with one Spark agg (equal_range, :216-232) or
 approxQuantile (equal_frequency, :210-215) and then calls a Python UDF once per value
@@ -17,6 +17,8 @@ import math
 import os
 import warnings
 from collections import OrderedDict
+
+import numpy as np
 
 from .. import _lib, engine, profile
 from ..frame import Column, ColumnFrame, as_frame
@@ -523,4 +525,327 @@ def imputation_MMM(spark, idf, list_of_cols="missing", drop_cols=[], method_type
         odf = _apply_plan(fr, plan, order)
     if print_impact:
         _impact(spark, odf, missing_df, list_of_cols, num_cols, cat_cols, missing_cols, output_mode).show(len(list_of_cols), False)
+    return odf
+
+
+# ---- scaling: z_standardization, IQR_standardization, normalization (reference transformers.py:965-1366) --------------
+#
+# The parameters come from the existing passes (moments for mean / stddev / min / max, the GK sketch of approxQuantile
+# for the quartiles) and the transform is one streaming pass (anv_scale_columns).  All parameter arithmetic is IEEE
+# double on the host, as in the reference's Python and Spark's JVM.  Semantics and deviations: DESIGN.md section 1.
+
+_SCALE_DIR = {"z": "z_standardization", "iqr": "IQR_standardization", "norm": "normalization"}
+_MINMAX_CLASS = "org.apache.spark.ml.feature.MinMaxScalerModel"
+_DOUBLE_MAX = 1.7976931348623157e308      # Scala's Double.MaxValue: an all-NaN feature's min in MinMaxScalerModel
+
+
+def _scale_cols(fr, list_of_cols, drop_cols, output_mode, what):
+    """The reference's argument checks, in its order; -> the columns (first-seen order), or None (warned: nothing to do)."""
+    num_cols = attributeType_segregation(fr)[0]
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        list_of_cols = num_cols
+    drop = _names(drop_cols)
+    cols = [c for c in dict.fromkeys(_names(list_of_cols)) if c not in drop]
+    if any(c not in num_cols for c in cols):
+        raise TypeError("Invalid input for Column(s)")
+    if not cols:
+        warnings.warn("No %s Performed - No numerical column(s) to transform" % what)
+        return None
+    if output_mode not in ("replace", "append"):
+        raise TypeError("Invalid input for output_mode")
+    sdt = dict(fr.dtypes)
+    for c in cols:
+        if sdt[c] not in _ANV_OF_SDTYPE:
+            raise TypeError("scaling of %s column %r is not supported on the device" % (sdt[c], c))
+    return cols
+
+
+def _save_param_model(model_path, kind, cols, params):
+    """parquet [feature: string, parameters: array<double>] at <model_path>/<kind> (elements may be null)."""
+    import pyarrow as pa
+    import pyarrow.parquet as pq
+    d = os.path.join(model_path, _SCALE_DIR[kind])
+    _clear_dir(d)
+    t = pa.table({"feature": pa.array(list(cols), pa.string()),
+                  "parameters": pa.array([[None if v is None else float(v) for v in p] for p in params],
+                                         pa.list_(pa.float64()))})
+    pq.write_table(t, os.path.join(d, "part-00000.snappy.parquet"), compression="snappy")
+    open(os.path.join(d, "_SUCCESS"), "w").close()
+
+
+def _load_param_model(model_path, kind, cols):
+    """`df_model.where(feature == c).select("parameters")...collect()[0]` per column; a missing column raises the
+    reference's IndexError."""
+    import pyarrow.parquet as pq
+    d = os.path.join(model_path, _SCALE_DIR[kind])
+    model = {}
+    for f in _spark_parts(d):
+        if f.endswith(".parquet"):
+            t = pq.read_table(f)
+            for a, p in zip(t.column("feature").to_pylist(), t.column("parameters").to_pylist()):
+                model.setdefault(a, p)
+    out = []
+    for c in cols:
+        if c not in model:
+            raise IndexError("list index out of range")
+        out.append(model[c])
+    return out
+
+
+def save_minmax_model(model_path, lo, hi, mins, maxs):
+    """Spark ML's MinMaxScalerModel directory at <model_path>/normalization: metadata/part-00000 (one JSON line) and
+    data/*.parquet (one row: originalMin, originalMax as dense vectors), each with a _SUCCESS marker."""
+    import json
+    import time
+    import uuid
+    import pyarrow as pa
+    import pyarrow.parquet as pq
+    d = os.path.join(model_path, _SCALE_DIR["norm"])
+    _clear_dir(d)
+    uid = "MinMaxScaler_" + uuid.uuid4().hex[:12]
+    meta = {"class": _MINMAX_CLASS, "timestamp": int(time.time() * 1000), "sparkVersion": "3.2.1", "uid": uid,
+            "paramMap": {"inputCol": "list_of_cols_vector", "outputCol": "list_of_cols_scaled"},
+            "defaultParamMap": {"min": float(lo), "max": float(hi), "outputCol": uid + "__output"}}
+    for sub in ("metadata", "data"):
+        os.makedirs(os.path.join(d, sub))
+        open(os.path.join(d, sub, "_SUCCESS"), "w").close()
+    with open(os.path.join(d, "metadata", "part-00000"), "w") as f:
+        f.write(json.dumps(meta) + "\n")
+    vec = pa.struct([pa.field("type", pa.int8(), False), pa.field("size", pa.int32()),
+                     pa.field("indices", pa.list_(pa.field("element", pa.int32(), False))),
+                     pa.field("values", pa.list_(pa.field("element", pa.float64(), False)))])
+
+    def dense(v):
+        return pa.array([{"type": 1, "size": None, "indices": None, "values": [float(x) for x in v]}], vec)
+    t = pa.table({"originalMin": dense(mins), "originalMax": dense(maxs)})
+    pq.write_table(t, os.path.join(d, "data", "part-00000.snappy.parquet"), compression="snappy")
+
+
+def _vector_values(v):
+    """A Spark ML vector struct {type, size, indices, values} -> list of doubles (dense: type 1; sparse: type 0)."""
+    if v["type"] == 1:
+        return [float(x) for x in v["values"]]
+    out = [0.0] * int(v["size"])
+    for i, x in zip(v["indices"], v["values"]):
+        out[i] = float(x)
+    return out
+
+
+def load_minmax_model(model_path):
+    """-> (lo, hi, originalMin, originalMax) of a MinMaxScalerModel directory (Spark's own or ours)."""
+    import json
+    import pyarrow.parquet as pq
+    d = os.path.join(model_path, _SCALE_DIR["norm"])
+    meta = json.loads(open(_spark_parts(os.path.join(d, "metadata"))[0]).readline())
+    pm, dm = meta.get("paramMap", {}), meta.get("defaultParamMap", {})
+    lo, hi = float(pm.get("min", dm.get("min", 0.0))), float(pm.get("max", dm.get("max", 1.0)))
+    rows = []
+    for f in _spark_parts(os.path.join(d, "data")):
+        if f.endswith(".parquet"):
+            rows += pq.read_table(f).to_pylist()
+    return lo, hi, _vector_values(rows[0]["originalMin"]), _vector_values(rows[0]["originalMax"])
+
+
+def _stddev(rec):
+    n = int(rec["n_valid"])
+    return math.sqrt(float(rec["m2"]) / (n - 1)) if n > 1 else None
+
+
+def _nan_free_moments(fr, cols):
+    """Moments over the non-null, non-NaN values: float columns whose mean is NaN (they hold NaN, or both infinities) take
+    theirs from the NaN-free view, like `_surrogates`.  -> (moments by name, the view, the columns read through it)."""
+    mom = profile.moments(fr, cols)
+    nan_cols = [c for c in cols if fr.column(c).anv_dtype in (_lib.ANV_F32, _lib.ANV_F64)
+                and math.isnan(float(mom[c]["mean"])) and int(mom[c]["n_valid"]) > 0]
+    view = _nan_view(fr, nan_cols)
+    out = dict(mom)
+    if nan_cols:
+        out.update(zip(nan_cols, engine.moments(view, nan_cols)))
+    return out, view, nan_cols
+
+
+def _quartiles(fr, cols):
+    """approxQuantile(cols, [0.25, 0.5, 0.75], 0.01), which skips NaN as well as null: [] for a column without a value."""
+    _, view, nan_cols = _nan_free_moments(fr, cols)
+    probs = [0.25, 0.5, 0.75]
+    q = dict(profile.quantiles(fr, [c for c in cols if c not in nan_cols], probs, profile.APPROX_QUANTILE_EPS))
+    if nan_cols:
+        q.update(profile.quantiles(view, nan_cols, probs, profile.APPROX_QUANTILE_EPS))
+    return [[] if any(v is None for v in q[c]) else [float(v) for v in q[c]] for c in cols]
+
+
+def _div_spec(a, b):
+    """`(col - a) / b` in Spark: a null parameter or a zero divisor (Divide returns null) -> None (an all-null column)."""
+    if a is None or b is None or b == 0:
+        return None
+    return (_lib.SCALE_DIV, _lib.ANV_F64, 0, float(a), float(b), 0.0)
+
+
+def minmax_spec(mn, mx, lo=0.0, hi=1.0):
+    """MinMaxScalerModel.transform of one feature: scale = (hi - lo) / (max - min); a zero scale (a constant column, or
+    an infinite range) maps every value to 0.5 * (hi - lo) + lo.  NaN results become null, the output is float."""
+    with np.errstate(divide="ignore", over="ignore", invalid="ignore"):
+        rng = np.float64(mx) - np.float64(mn)
+        scale = float(np.float64(hi - lo) / rng) if rng != 0 else 0.0
+    if scale != 0:
+        return (_lib.SCALE_AFFINE, _lib.ANV_F32, _lib.SCALE_NAN_TO_NULL, float(mn), scale, float(lo))
+    return (_lib.SCALE_CONST, _lib.ANV_F32, _lib.SCALE_NAN_TO_NULL, 0.0, 0.0, 0.5 * (hi - lo) + lo)
+
+
+def _apply_scaling(fr, cols, specs, output_mode):
+    """Write the scaled columns (spec None: an all-null double column) -> new frame.  "replace": each takes its source's
+    name and position; "append": `<c>_scaled` after all existing columns, in list order."""
+    run = [i for i, s in enumerate(specs) if s is not None]
+    data, valid, nulls = engine.scale_columns(fr, [cols[i] for i in run], [specs[i] for i in run])
+    made = {}
+    for k, i in enumerate(run):
+        src = fr.column(cols[i])
+        od = specs[i][1]
+        if specs[i][2] & _lib.SCALE_NAN_TO_NULL:
+            v, nc = valid[k], int(nulls[k])
+        else:
+            v, nc = src.device()[1], src.null_count
+        made[cols[i]] = Column(cols[i], _SDTYPE_OF_ANV[od], fr.n_rows, dev=data[k], dev_valid=v, anv_dtype=od, null_count=nc)
+    for i, s in enumerate(specs):
+        if s is None:
+            d, _ = fr.column(cols[i]).device()
+            torch = _lib.require_cuda()
+            made[cols[i]] = Column(cols[i], "double", fr.n_rows, dev=torch.zeros(max(fr.n_rows, 1), dtype=torch.float64,
+                                                                                  device=d.device)[:fr.n_rows],
+                                   dev_valid=torch.zeros(max((fr.n_rows + 31) // 32, 1), dtype=torch.int32, device=d.device),
+                                   anv_dtype=_lib.ANV_F64, null_count=fr.n_rows)
+    new = OrderedDict()
+    for n in fr.columns:
+        new[n] = made[n] if output_mode == "replace" and n in made else fr.column(n)
+    if output_mode == "append":
+        for c in cols:
+            if c in made:
+                col = made[c]
+                col.name = c + "_scaled"
+                new[col.name] = col
+    return ColumnFrame(new, fr.n_rows)
+
+
+def _scaled_frame(fr, cols, specs, output_mode):
+    if getattr(fr, "is_partitioned", False):
+        schema = _apply_scaling(fr._schema, cols, specs, output_mode)
+        return fr.map_chunks(schema, lambda ch: _apply_scaling(ch, cols, specs, output_mode))
+    return _apply_scaling(fr, cols, specs, output_mode)
+
+
+def _describe_value(v, sdtype):
+    from ..shared.utils import jvm_double_str
+    if v is None or (v != v and sdtype in ("int", "bigint", "long")):
+        return "null"
+    if sdtype in ("int", "bigint", "long"):
+        return str(int(v))
+    if sdtype == "float":                  # Float.toString: the shortest float32 digits
+        return jvm_double_str(float(str(np.float32(v))))
+    return jvm_double_str(v)
+
+
+def describe(fr, cols):
+    """`idf.select(cols).describe()` (count, mean, stddev, min, max as strings) from the moments pass."""
+    import pandas as pd
+    from ..result import ResultFrame
+    mom = profile.moments(fr, cols)
+    sdt = dict(fr.dtypes)
+    rows = {"count": [], "mean": [], "stddev": [], "min": [], "max": []}
+    for c in cols:
+        r = mom[c]
+        n = int(r["n_valid"])
+        rows["count"].append(str(n))
+        rows["mean"].append(_describe_value(float(r["mean"]) if n else None, "double"))
+        rows["stddev"].append(_describe_value(_stddev(r), "double"))
+        rows["min"].append(_describe_value(float(r["min"]) if n else None, sdt[c]))
+        rows["max"].append(_describe_value(float(r["max"]) if n else None, sdt[c]))
+    return ResultFrame(pd.DataFrame([[k] + v for k, v in rows.items()], columns=["summary"] + list(cols)))
+
+
+def _print_impact(fr, odf, cols, out_cols):
+    print("Before: ")
+    describe(fr, cols).show(5, False)
+    print("After: ")
+    describe(odf, out_cols).show(5, False)
+
+
+def z_standardization(spark, idf, list_of_cols="all", drop_cols=[], pre_existing_model=False, model_path="NA",
+                      output_mode="replace", print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:965-1099): (x - mean) / stddev as a
+    double column that keeps the source's nulls."""
+    fr = as_frame(idf)
+    cols = _scale_cols(fr, list_of_cols, drop_cols, output_mode, "Standardization")
+    if cols is None:
+        return fr
+    excluded = []
+    if pre_existing_model:
+        params = _load_param_model(model_path, "z", cols)
+    else:
+        mom = profile.moments(fr, cols)
+        params = []
+        for c in cols:
+            n = int(mom[c]["n_valid"])
+            mean, sd = (float(mom[c]["mean"]) if n else None), _stddev(mom[c])
+            params.append([mean if mean else None, sd if sd else None])   # `float(mean) if mean else None`
+            if not sd or round(sd, 5) == 0.0:
+                excluded.append(c)
+    if excluded:
+        warnings.warn("The following column(s) are excluded from standardization because the standard deviation is zero:"
+                      + str(excluded))
+    kept = [c for c in cols if c not in excluded]
+    specs = [_div_spec(p[0], p[1]) for c, p in zip(cols, params) if c not in excluded]
+    odf = _scaled_frame(fr, kept, specs, output_mode)
+    if not pre_existing_model and model_path != "NA":
+        _save_param_model(model_path, "z", cols, params)
+    if print_impact:
+        _print_impact(fr, odf, cols, cols if output_mode == "replace" else [c + "_scaled" for c in kept])
+    return odf
+
+
+def IQR_standardization(spark, idf, list_of_cols="all", drop_cols=[], pre_existing_model=False, model_path="NA",
+                        output_mode="replace", print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:1102-1230): (x - p50) / (p75 - p25)
+    with the quartiles of approxQuantile(..., 0.01), as a double column that keeps the source's nulls."""
+    fr = as_frame(idf)
+    cols = _scale_cols(fr, list_of_cols, drop_cols, output_mode, "Standardization")
+    if cols is None:
+        return fr
+    params = _load_param_model(model_path, "iqr", cols) if pre_existing_model else _quartiles(fr, cols)
+    excluded = [c for c, p in zip(cols, params) if len(p) == 0 or round(p[0], 5) == round(p[2], 5)]
+    if excluded:
+        warnings.warn("The following column(s) are excluded from standardization because the 75th and 25th percentiles "
+                      "are the same:" + str(excluded))
+    kept = [c for c in cols if c not in excluded]
+    specs = [_div_spec(p[1], None if p[2] is None or p[0] is None else p[2] - p[0])
+             for c, p in zip(cols, params) if c not in excluded]
+    odf = _scaled_frame(fr, kept, specs, output_mode)
+    if not pre_existing_model and model_path != "NA":
+        _save_param_model(model_path, "iqr", cols, params)
+    if print_impact:
+        _print_impact(fr, odf, cols, cols if output_mode == "replace" else [c + "_scaled" for c in kept])
+    return odf
+
+
+def normalization(idf, list_of_cols="all", drop_cols=[], pre_existing_model=False, model_path="NA", output_mode="replace",
+                  print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:1233-1366): Spark ML's MinMaxScaler to
+    [0, 1] over the non-null, non-NaN values, as a float column; NaN (input or result) becomes null."""
+    fr = as_frame(idf)
+    cols = _scale_cols(fr, list_of_cols, drop_cols, output_mode, "Normalization")
+    if cols is None:
+        return fr
+    if pre_existing_model:
+        lo, hi, mins, maxs = load_minmax_model(model_path)
+        if len(mins) != len(cols) or len(maxs) != len(cols):
+            raise ValueError("normalization model has %d features, the column list %d" % (len(mins), len(cols)))
+    else:
+        lo, hi = 0.0, 1.0
+        mom, _, _ = _nan_free_moments(fr, cols)
+        mins = [float(mom[c]["min"]) if int(mom[c]["n_valid"]) else _DOUBLE_MAX for c in cols]
+        maxs = [float(mom[c]["max"]) if int(mom[c]["n_valid"]) else -_DOUBLE_MAX for c in cols]
+        if model_path != "NA":
+            save_minmax_model(model_path, lo, hi, mins, maxs)
+    odf = _scaled_frame(fr, cols, [minmax_spec(a, b, lo, hi) for a, b in zip(mins, maxs)], output_mode)
+    if print_impact:
+        _print_impact(fr, odf, cols, cols if output_mode == "replace" else [c + "_scaled" for c in cols])
     return odf

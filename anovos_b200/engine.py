@@ -847,3 +847,49 @@ def valid_not_nan(frame: ColumnFrame, names):
           n_nan.data_ptr(), _stream(), nbytes=input_bytes(frame, names))
     launch_count += 1
     return words[:, :n_words], _host(n_nan).view(np.int64)[:len(names)].copy()
+
+
+# ---- scaling -------------------------------------------------------------------------------------
+
+_SCALE_SPEC_DT = np.dtype([("mode", "<i4"), ("out_dtype", "<i4"), ("flags", "<i4"), ("reserved", "<i4"),
+                           ("a", "<f8"), ("b", "<f8"), ("c", "<f8")])
+
+
+def scale_columns(frame: ColumnFrame, names, specs):
+    """anv_scale_columns: specs = one (mode, out anv dtype, flags, a, b, c) per name (_lib.SCALE_*).
+    -> (list of CUDA tensors [n_rows] in the output dtype, list of int32 bitmap tensors [ceil(n_rows/32)] for the
+    NAN_TO_NULL columns and None for the others (which keep the source's validity), int64 ndarray of null counts)."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names, specs = list(names), list(specs)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: scale_columns(frame, names[lo:hi], specs[lo:hi]), len(names))
+    sp = np.zeros(len(names), _SCALE_SPEC_DT)
+    outs, ptrs = [], np.zeros(len(names), np.uint64)
+    padded = (frame.n_rows + 3) // 4 * 4
+    for i, (n, (mode, od, fl, a, b, c)) in enumerate(zip(names, specs)):
+        if mode not in (_lib.SCALE_DIV, _lib.SCALE_AFFINE, _lib.SCALE_CONST) or od not in (_lib.ANV_F32, _lib.ANV_F64) \
+                or frame.column(n).anv_dtype not in _NP_OF_ANV or fl & ~_lib.SCALE_NAN_TO_NULL:
+            raise ValueError("scale_columns: column %r: no scale mode %r to dtype %r with flags %r" % (n, mode, od, fl))
+        sp[i] = (mode, od, fl, 0, a, b, c)
+        t = torch.empty(max(padded, 4), dtype=getattr(torch, _TORCH_OF_ANV[od]), device="cuda")
+        outs.append(t)
+        ptrs[i] = t.data_ptr()
+    n_words = (frame.n_rows + 31) // 32
+    flagged = [bool(s[2] & _lib.SCALE_NAN_TO_NULL) for s in specs]
+    words = torch.zeros((max(len(names), 1), max(n_words, 1)), dtype=torch.int32, device="cuda") if any(flagged) else None
+    if not names or not frame.n_rows:
+        return [t[:frame.n_rows] for t in outs], [None if words is None else words[i, :n_words] if f else None
+                                                  for i, f in enumerate(flagged)], np.zeros(len(names), np.int64)
+    nulls = _dev_bytes(len(names) * 8)
+    desc, keep = frame.descriptors(names)
+    nbytes = input_bytes(frame, names)
+    if timer is not None:
+        nbytes += sum(frame.n_rows * t.element_size() + (n_words * 4 if f else 0) for t, f in zip(outs, flagged))
+    dspecs, dptrs = _to_dev(sp), _to_dev(ptrs)          # held until the launch is enqueued
+    _call(L.anv_scale_columns, "anv_scale_columns", desc.data_ptr(), dspecs.data_ptr(), dptrs.data_ptr(),
+          None if words is None else words.data_ptr(), nulls.data_ptr(), len(names), frame.n_rows, _stream(), nbytes=nbytes)
+    launch_count += 1
+    valid = [words[i, :n_words] if f else None for i, f in enumerate(flagged)]
+    return [t[:frame.n_rows] for t in outs], valid, _host(nulls).view(np.int64)[:len(names)].copy()

@@ -281,6 +281,34 @@ int anv_impute_fill(const anv_column_t* cols, const anv_impute_spec_t* specs, vo
 int anv_valid_not_nan(const anv_column_t* cols, int n_cols, int64_t n_rows, uint32_t* out_validity, int64_t* n_nan,
                       void* stream);
 
+/* ---- scaling (z_standardization, IQR_standardization, normalization; data_transformer/transformers.py:965-1366).
+ * anv_scale_columns: one streaming pass per column writes out[r] for every row r, in IEEE double with each operation
+ * rounded on its own (no FMA contraction, no reciprocal multiply):
+ *   ANV_SCALE_DIV     out = (double(x) - a) / b
+ *   ANV_SCALE_AFFINE  out = (double(x) - a) * b + c
+ *   ANV_SCALE_CONST   out = c
+ * double(x) is the plain conversion of an F32 / F64 / I32 / I64 input (a bigint beyond 2^53 rounds to nearest); an F32
+ * out_dtype rounds the double result to nearest.  ANV_SCALE_NAN_TO_NULL: a row whose input or result is NaN is null.
+ * Null rows are written as 0.  Under the flag, out_validity + c * ceil(n_rows/32) gets the output bitmap of column c
+ * (source valid, input not NaN, result not NaN; bits past n_rows are 0).  Without the flag no bitmap is written: the output keeps the source's validity.  null_counts
+ * [dev] n_cols int64 (zeroed by the library): the null rows of each output.  A spec whose mode or out_dtype is not one of
+ * the above leaves its column unwritten.
+ * specs [dev] n_cols; out_ptrs [dev] n_cols device pointers, each 16-byte aligned with room for n_rows rounded up to a
+ * multiple of 4 elements; out_validity [dev] n_cols * ceil(n_rows/32) words, or NULL when no spec has NAN_TO_NULL. */
+#define ANV_SCALE_DIV 0
+#define ANV_SCALE_AFFINE 1
+#define ANV_SCALE_CONST 2
+#define ANV_SCALE_NAN_TO_NULL 1
+typedef struct {
+  int32_t mode;      /* ANV_SCALE_DIV / AFFINE / CONST */
+  int32_t out_dtype; /* ANV_F32 or ANV_F64 */
+  int32_t flags;     /* ANV_SCALE_NAN_TO_NULL */
+  int32_t reserved;
+  double a, b, c;
+} anv_scale_spec_t;
+int anv_scale_columns(const anv_column_t* cols, const anv_scale_spec_t* specs, void* const* out_ptrs, uint32_t* out_validity,
+                      int64_t* null_counts, int n_cols, int64_t n_rows, void* stream);
+
 /* ---- Spark's Bernoulli row sampler (the DEFAULT path of drift_detector.statistics: use_sampling=True ->
  *      data_sampling.py:122-149 `idf.sample(False, fraction, seed)` / `stat.sampleBy("merge", fractions, seed)`,
  *      drift_detector.py:187-211).  One partition per call: Spark seeds XORShiftRandom with seed + partitionIndex,

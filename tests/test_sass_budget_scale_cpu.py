@@ -1,0 +1,21 @@
+"""The scale kernel in the built library (no GPU: cuobjdump reads the sm_90a SASS): it is a streaming pass, so it must
+not spill to local memory and must move its values with 128-bit global loads and stores."""
+import re
+import subprocess
+
+import pytest
+
+from test_sass_budget_cpu import _cuobjdump, _sass
+
+FUN = "_ZN3anv12scale_kernelEPK12anv_column_tPK16anv_scale_spec_tPKPvPjPyl"
+
+
+def test_scale_kernel_streams_without_spills():
+    if _cuobjdump() is None:
+        pytest.skip("cuobjdump not found")
+    from anovos_b200 import build
+    ins = _sass(build.build(), FUN)
+    assert ins, "no SASS for " + FUN
+    assert not [i for i in ins if re.search(r"\b(LDL|STL)\b", i)]
+    assert any(re.match(r"LDG\.E\.[A-Z.]*128", i) for i in ins)
+    assert any(re.match(r"STG\.E\.[A-Z.]*128", i) for i in ins)
