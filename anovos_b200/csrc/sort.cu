@@ -1432,7 +1432,7 @@ __global__ void __launch_bounds__(ANV_BLOCK, 4) pc_coarse_kernel(const PcParams 
 __global__ void __launch_bounds__(256) pc_chunks_kernel(const PcParams P) {
   const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t t = tid < P.G ? P.totals[(size_t)c * 256 + tid] : 0u;
-  const uint32_t k = (t + PC_CHUNK - 1) / PC_CHUNK;
+  const uint32_t k = t / PC_CHUNK + (t % PC_CHUNK != 0u);   // (t + PC_CHUNK - 1) would wrap for t > 2^32 - PC_CHUNK
   uint32_t it = t, ik = k;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
@@ -1506,7 +1506,7 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_fine_kernel(const PcParams P) {
   const int g = s_g;
   const uint32_t gend = gs[g + 1];
   const uint32_t p0 = gs[g] + ((uint32_t)b - cb[g]) * PC_CHUNK;
-  const uint32_t p1 = min(p0 + PC_CHUNK, gend);
+  const uint32_t p1 = p0 + min((uint32_t)PC_CHUNK, gend - p0);   // p0 + PC_CHUNK may pass 2^32 in a column of < 2^32 keys
   const uint32_t* O = P.tile_hist + ((size_t)c * 256 + g) * P.n_tiles;
   const uint16_t* TS = P.tile_start + ((size_t)c * 256 + g) * P.n_tiles;
   const uint32_t* __restrict__ src = P.keys[0] + (size_t)c * P.stride;
@@ -1520,10 +1520,13 @@ __global__ void __launch_bounds__(ANV_BLOCK) pc_fine_kernel(const PcParams P) {
     }
     __syncthreads();
     const uint32_t wlo = max(p0, sO[0]), whi = min(p1, sO[PC_WIN]);
-    for (uint32_t q = wlo + tid; q < whi; q += ANV_BLOCK) {
+    // positions relative to p0 (< PC_CHUNK): q += ANV_BLOCK could wrap past 2^32 near the end of a long column
+    const uint32_t i1 = whi > p0 ? whi - p0 : 0u;
+    for (uint32_t i = wlo - p0 + tid; i < i1; i += ANV_BLOCK) {
+      const uint32_t q = p0 + i;
       int lo = 0, hi = PC_WIN - 1;                  // last i with sO[i] <= q
       while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (sO[mid] <= q) lo = mid; else hi = mid - 1; }
-      pc_cp_async4(&sk[q - p0], src + (size_t)(t0 + lo) * SORT_TILE + sTS[lo] + (q - sO[lo]));   // nothing waits for it
+      pc_cp_async4(&sk[i], src + (size_t)(t0 + lo) * SORT_TILE + sTS[lo] + (q - sO[lo]));   // nothing waits for it
     }
     const bool done = whi >= p1;
     __syncthreads();                                // sO / sTS are refilled by the next round

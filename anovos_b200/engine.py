@@ -454,9 +454,17 @@ def select_ranks(frame: ColumnFrame, names, ranks):
 
 # ---- sort-based exact mode / distinct --------------------------------------------------------
 
+EXACT_MAX_ROWS = (1 << 32) - 1    # rows one exact mode / distinct call counts: multiplicities and row numbers are 32-bit
 SORT_WORKSPACE_BUDGET = 24 << 30  # bytes of scratch one sort batch may use
 sort_algorithm = "partition"      # "partition": F32 / I32 columns with <= 16 ranks take the bucket count; "lsd": every column sorts
 FUSED_HLL = True                  # sort_mode_distinct(..., hll_p=p) also returns the HLL++ registers (one hash per distinct value)
+
+
+def refuse_exact_rows(n_rows, what):
+    """AnvError for frames of 2^32 rows or more, which the exact mode / distinct counts of one call cannot count."""
+    if n_rows > EXACT_MAX_ROWS:
+        raise _lib.AnvError("%s: frames of 2^32 rows or more are not supported (%d rows): the exact mode and distinct "
+                            "counts are 32-bit; use the approximate distinct count (HLL++) instead" % (what, n_rows))
 
 
 def _mode_distinct_batch_size(frame, n_cols, per_col_bytes):
@@ -482,7 +490,9 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
     F32 / I32 columns with at most 16 ranks go through the two-level bucket count (anv_mode_distinct_partition_hll: no
     sort, ~4 words of traffic per key - DESIGN.md section 3); 64-bit columns, longer rank lists and sort_algorithm = "lsd"
     take the batched LSD radix sort (anv_mode_distinct).  All column batches of a call are enqueued back to back on the
-    stream into one workspace (stream order makes the reuse safe) and the results come back in ONE device-to-host copy."""
+    stream into one workspace (stream order makes the reuse safe) and the results come back in ONE device-to-host copy.
+    Frames of more than EXACT_MAX_ROWS rows raise AnvError before anything is allocated."""
+    refuse_exact_rows(frame.n_rows, "sort_mode_distinct")
     if getattr(frame, "is_partitioned", False):
         return frame.sort_mode_distinct(names, ranks)
     global launch_count

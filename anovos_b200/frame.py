@@ -91,15 +91,26 @@ def _pack_validity(valid_bool: np.ndarray) -> np.ndarray:
     return bits.view(np.int32)
 
 
+_PACK_BLOCK_ROWS = 1 << 26      # rows packed per step of pack_bits_device: bounds its scratch at about 2 bytes per row of a step
+
+
 def pack_bits_device(bits):
-    """bool CUDA tensor [n] -> Arrow LSB-first validity bitmap as int32 words on the device."""
+    """bool tensor [n] -> Arrow LSB-first validity bitmap as int32 words, on the tensor's device.  Every 8 rows become one
+    byte (a sum of the rows weighted by 1, 2, ..., 128 in uint8) and four bytes one little-endian word, step by step, so a
+    mask of billions of rows needs about n / 8 bytes of output and a few bytes per row of one step, not an int64 per row."""
     import torch
     n = int(bits.numel())
     words = (n + 31) // 32
-    padded = torch.zeros(words * 32, dtype=torch.int64, device=bits.device)
-    padded[:n] = bits.to(torch.int64)
-    w = (padded.view(words, 32) << torch.arange(32, device=bits.device, dtype=torch.int64)).sum(dim=1)
-    return (w & 0xFFFFFFFF).to(torch.int64).where(w < (1 << 31), w - (1 << 32)).to(torch.int32)
+    out = torch.zeros(max(words, 1) * 4, dtype=torch.uint8, device=bits.device)
+    weights = torch.tensor([1 << i for i in range(8)], dtype=torch.uint8, device=bits.device)
+    flat = bits.reshape(-1)
+    for r0 in range(0, n, _PACK_BLOCK_ROWS):
+        r1 = min(r0 + _PACK_BLOCK_ROWS, n)
+        blk = flat[r0:r1].to(torch.uint8)
+        if (r1 - r0) % 8:
+            blk = torch.cat([blk, blk.new_zeros(8 - (r1 - r0) % 8)])
+        out[r0 // 8:r0 // 8 + blk.numel() // 8] = (blk.view(-1, 8) * weights).sum(dim=1, dtype=torch.uint8)
+    return out.view(torch.int32)[:words]
 
 
 def _arrow_validity_words(arr):

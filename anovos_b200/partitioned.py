@@ -435,6 +435,7 @@ class PartitionedFrame:
         columns of its block over NVLink), each rank sorts its block and the small per-column results are
         all-gathered, so every rank returns the full answer."""
         from . import engine
+        engine.refuse_exact_rows(self.n_rows, "sort_mode_distinct")     # before anything is materialized
         torch = _lib.require_cuda()
         names = list(names)
         need = sum(self.n_rows * (8 if self.column(n).anv_dtype in (_lib.ANV_F64, _lib.ANV_I64) else 4) for n in names)
