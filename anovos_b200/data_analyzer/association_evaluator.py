@@ -10,15 +10,15 @@ the host.  `monotonicity_check=1` (monotonic_binning) is not part of this build.
 from __future__ import annotations
 
 import math
-from collections import OrderedDict
 
 import numpy as np
 import pandas as pd
 
 from .. import engine
 from ..data_transformer.transformers import compute_cutoffs
-from ..frame import Column, ColumnFrame, as_frame
+from ..frame import as_frame
 from ..result import ResultFrame
+from ..shared.label_classes import label_bitmaps as _label_bitmaps, masked as _masked
 from ..shared.utils import attributeType_segregation
 
 _DEFAULT_ENC = {"bin_method": "equal_frequency", "bin_size": 10, "monotonicity_check": 0}
@@ -28,53 +28,6 @@ def _names(x):
     if isinstance(x, str):
         return [s.strip() for s in x.split("|")]
     return list(x)
-
-
-def _pack_bits(mask):
-    """bool CUDA tensor [n] -> int32 Arrow bitmap words (LSB-first)."""
-    import torch
-    n = mask.numel()
-    pad = (-n) % 32
-    if pad:
-        mask = torch.cat([mask, torch.zeros(pad, dtype=torch.bool, device=mask.device)])
-    w = (mask.view(-1, 32).to(torch.int64) << torch.arange(32, device=mask.device, dtype=torch.int64)).sum(dim=1)
-    return ((w + (1 << 31)) % (1 << 32) - (1 << 31)).to(torch.int32)
-
-
-def _unpack_bits(words, n):
-    import torch
-    rows = torch.arange(n, device=words.device)
-    return ((words[rows >> 5] >> (rows & 31).to(torch.int32)) & 1).bool()
-
-
-def _label_bitmaps(fr: ColumnFrame, label_col, event_label):
-    """-> (event words, non-event words, n_event): rows with label == event_label / label != event_label
-    (a null label is in neither class)."""
-    import torch
-    col = fr.column(label_col)
-    d, v = col.device()
-    if col.kind == "cat":
-        try:
-            code = col.dictionary.index(str(event_label))
-        except ValueError:
-            code = -1
-        is_ev = d == code
-    else:
-        is_ev = d.to(torch.float64) == float(event_label)
-    valid = _unpack_bits(v, fr.n_rows) if v is not None else torch.ones(fr.n_rows, dtype=torch.bool, device=d.device)
-    ev, nev = is_ev & valid, (~is_ev) & valid
-    return _pack_bits(ev), _pack_bits(nev), int(ev.sum().item())
-
-
-def _masked(fr: ColumnFrame, names, words) -> ColumnFrame:
-    """Same columns with validity := validity AND words (rows outside the class become "null")."""
-    cols = OrderedDict()
-    for n in names:
-        c = fr.column(n)
-        d, v = c.device()
-        nv = words if v is None else (v & words)
-        cols[n] = Column(n, c.sdtype, fr.n_rows, dev=d, dev_valid=nv, anv_dtype=c.anv_dtype, dictionary=c.dictionary)
-    return ColumnFrame(cols, fr.n_rows)
 
 
 def _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_configs):

@@ -849,3 +849,580 @@ def normalization(idf, list_of_cols="all", drop_cols=[], pre_existing_model=Fals
     if print_impact:
         _print_impact(fr, odf, cols, cols if output_mode == "replace" else [c + "_scaled" for c in cols])
     return odf
+
+
+# ---- categorical encoding: cat_to_num_unsupervised, cat_to_num_supervised, outlier_categories ------------------------
+# (reference transformers.py:428-962, 3489-3671)
+#
+# Every fit reads the per-category counts of the code histogram pass (profile.code_counts, merged over row chunks); the
+# supervised encoder adds one masked pass for the event rows.  Every transform is one streaming pass: anv_code_map looks
+# each row's code up in a per-column table (label index, rate or new code), anv_one_hot expands it into n + 1 dense int
+# columns.  Dictionaries are not sorted in general (imputation_MMM appends its fill strings), so every order below comes
+# from an explicit sort of the categories with a nonzero count, in UTF-8 byte order as Spark compares strings.  Semantics
+# and deviations: DESIGN.md section 1.
+
+_OUTLIER = "outlier_categories"
+_INDEX_ORDERS = ("frequencyDesc", "frequencyAsc", "alphabetDesc", "alphabetAsc")
+_PRINT_TYPE = {"string": "string", "int": "integer", "bigint": "long", "long": "long", "float": "float",
+               "double": "double"}
+
+
+def _utf8(s):
+    return s.encode("utf-8")
+
+
+def _split(x):
+    return [s.strip() for s in x.split("|")] if isinstance(x, str) else list(x)
+
+
+def _present(fr, cols):
+    """-> {col: [(category, count)]} over the categories with a nonzero count, and {col: null rows}."""
+    cc = profile.code_counts(fr, cols)
+    out, nulls = {}, {}
+    for c in cols:
+        h, dic = cc[c], fr.column(c).dictionary
+        out[c] = [(dic[k], int(h[k + 1])) for k in range(len(dic)) if int(h[k + 1]) > 0]
+        nulls[c] = int(h[0])
+    return out, nulls
+
+
+def string_indexer_labels(counts, index_order):
+    """StringIndexer (Spark 3) labels of [(category, count)]: frequency orders break ties by label ascending."""
+    if index_order == "frequencyDesc":
+        key = lambda t: (-t[1], _utf8(t[0]))          # noqa: E731
+    elif index_order == "frequencyAsc":
+        key = lambda t: (t[1], _utf8(t[0]))           # noqa: E731
+    else:
+        key = lambda t: _utf8(t[0])                   # noqa: E731
+    labels = [t[0] for t in sorted(counts, key=key)]
+    return labels[::-1] if index_order == "alphabetDesc" else labels
+
+
+def _label_index(dictionary, labels):
+    """int32 table of len(dictionary) + 1 entries: a category's position in `labels`, n for one it lacks and the null slot
+    (StringIndexer's handleInvalid="keep")."""
+    pos = {s: i for i, s in enumerate(labels)}
+    return np.array([pos.get(s, len(labels)) for s in dictionary] + [len(labels)], np.int32)
+
+
+def _write_json_part(d, obj):
+    import json
+    os.makedirs(d)
+    with open(os.path.join(d, "part-00000"), "w") as f:
+        f.write(json.dumps(obj) + "\n")
+    open(os.path.join(d, "_SUCCESS"), "w").close()
+
+
+def _read_json_part(d):
+    import json
+    return json.loads(open(_spark_parts(d)[0]).readline())
+
+
+def save_indexer_model(model_path, cols, labels, index_order):
+    """Spark 3 StringIndexerModel directory at <model_path>/cat_to_num_unsupervised/indexer: metadata/part-00000 (one
+    JSON line) and data/*.parquet (one row, labelsArray: array<array<string>>)."""
+    import time
+    import uuid
+    import pyarrow as pa
+    import pyarrow.parquet as pq
+    d = os.path.join(model_path, "cat_to_num_unsupervised", "indexer")
+    _clear_dir(d)
+    uid = "StringIndexer_" + uuid.uuid4().hex[:12]
+    _write_json_part(os.path.join(d, "metadata"), {
+        "class": "org.apache.spark.ml.feature.StringIndexerModel", "timestamp": int(time.time() * 1000),
+        "sparkVersion": "3.2.1", "uid": uid,
+        "paramMap": {"inputCols": list(cols), "outputCols": [c + "_index" for c in cols], "stringOrderType": index_order,
+                     "handleInvalid": "keep"},
+        "defaultParamMap": {"outputCol": uid + "__output", "stringOrderType": "frequencyDesc", "handleInvalid": "error"}})
+    os.makedirs(os.path.join(d, "data"))
+    t = pa.table({"labelsArray": pa.array([[list(x) for x in labels]], pa.list_(pa.list_(pa.string())))})
+    pq.write_table(t, os.path.join(d, "data", "part-00000.snappy.parquet"), compression="snappy")
+    open(os.path.join(d, "data", "_SUCCESS"), "w").close()
+
+
+def load_indexer_model(model_path):
+    """-> {input col: labels} of a StringIndexerModel directory (Spark 3's own or ours)."""
+    import pyarrow.parquet as pq
+    d = os.path.join(model_path, "cat_to_num_unsupervised", "indexer")
+    pm = _read_json_part(os.path.join(d, "metadata")).get("paramMap", {})
+    ins = pm.get("inputCols") or [pm["inputCol"]]
+    rows = []
+    for f in _spark_parts(os.path.join(d, "data")):
+        if f.endswith(".parquet"):
+            rows += pq.read_table(f).to_pylist()
+    labels = rows[0]["labelsArray"] if "labelsArray" in rows[0] else [rows[0]["labels"]]
+    return dict(zip(ins, labels))
+
+
+def save_onehot_model(model_path, cols):
+    """The OneHotEncoder estimator at <model_path>/cat_to_num_unsupervised/encoder: metadata/part-00000 only."""
+    import time
+    import uuid
+    d = os.path.join(model_path, "cat_to_num_unsupervised", "encoder")
+    _clear_dir(d)
+    uid = "OneHotEncoder_" + uuid.uuid4().hex[:12]
+    _write_json_part(os.path.join(d, "metadata"), {
+        "class": "org.apache.spark.ml.feature.OneHotEncoder", "timestamp": int(time.time() * 1000),
+        "sparkVersion": "3.2.1", "uid": uid,
+        "paramMap": {"inputCols": [c + "_index" for c in cols], "outputCols": [c + "_vec" for c in cols],
+                     "handleInvalid": "keep"},
+        "defaultParamMap": {"outputCol": uid + "__output", "dropLast": True, "handleInvalid": "error"}})
+
+
+def _free_device_bytes():
+    """Free device memory, counting what torch's allocator holds unused."""
+    import torch
+    free, _ = torch.cuda.mem_get_info()
+    return int(free) + int(torch.cuda.memory_reserved()) - int(torch.cuda.memory_allocated())
+
+
+def _apply_label(fr, cols, labels, output_mode):
+    tables = [_label_index(fr.column(c).dictionary, labels[c]) for c in cols]
+    data, _, _ = engine.code_map(fr, cols, tables, [None] * len(cols))
+    made = OrderedDict()
+    for c, d in zip(cols, data):
+        src = fr.column(c)
+        name = c if output_mode == "replace" else c + "_index"
+        made[name] = Column(name, "int", fr.n_rows, dev=d, dev_valid=src.device()[1], anv_dtype=_lib.ANV_I32,
+                            null_count=src.null_count)
+    new = OrderedDict((n, made[n] if n in made else fr.column(n)) for n in fr.columns)
+    for n, col in made.items():
+        new.setdefault(n, col)
+    return ColumnFrame(new, fr.n_rows)
+
+
+def _apply_onehot(fr, cols, labels, output_mode):
+    stride = engine.one_hot_stride(fr.n_rows)
+    free, need = _free_device_bytes() if fr.n_rows else 0, 0
+    for c in cols:                                   # one engine.one_hot call allocates the outputs of every column
+        need += (len(labels[c]) + 1) * stride * 4
+        if fr.n_rows and need > free:
+            raise _lib.AnvError("one-hot encoding of column %r needs %d output columns; with the columns before it that "
+                                "is %.1f GB of device memory, more than the %.1f GB free: drop columns, lower "
+                                "cardinality_threshold or cap the categories with outlier_categories"
+                                % (c, len(labels[c]) + 1, need / 1e9, free / 1e9))
+    idx = [_label_index(fr.column(c).dictionary, labels[c]) for c in cols]
+    outs = engine.one_hot(fr, cols, idx, [len(labels[c]) + 1 for c in cols])
+    new = OrderedDict((n, fr.column(n)) for n in fr.columns if not (output_mode == "replace" and n in cols))
+    for c, o in zip(cols, outs):
+        for j in range(len(labels[c]) + 1):
+            name = "%s_%d" % (c, j)
+            new[name] = Column(name, "int", fr.n_rows, dev=o[j], anv_dtype=_lib.ANV_I32, null_count=0)
+    return ColumnFrame(new, fr.n_rows)
+
+
+def _per_chunk(fr, fn):
+    if getattr(fr, "is_partitioned", False):
+        return fr.map_chunks(fn(fr._schema), fn)
+    return fn(fr)
+
+
+def _summary_value(v, sdtype):
+    return "null" if v is None else _describe_value(v, sdtype)
+
+
+def summary_count_min_max(fr, cols):
+    """`idf.select(cols).summary("count", "min", "max")`: strings compare in UTF-8 order, numbers through the moments."""
+    import pandas as pd
+    from ..result import ResultFrame
+    cat = [c for c in cols if fr.column(c).kind == "cat"]
+    num = [c for c in cols if c not in cat]
+    present, _ = _present(fr, cat) if cat else ({}, {})
+    mom = profile.moments(fr, num) if num else {}
+    sdt = dict(fr.dtypes)
+    rows = {"count": [], "min": [], "max": []}
+    for c in cols:
+        if c in present:
+            keys = sorted((k for k, _ in present[c]), key=_utf8)
+            rows["count"].append(str(sum(n for _, n in present[c])))
+            rows["min"].append(keys[0] if keys else "null")
+            rows["max"].append(keys[-1] if keys else "null")
+        else:
+            n = int(mom[c]["n_valid"])
+            rows["count"].append(str(n))
+            rows["min"].append(_summary_value(float(mom[c]["min"]) if n else None, sdt[c]))
+            rows["max"].append(_summary_value(float(mom[c]["max"]) if n else None, sdt[c]))
+    return ResultFrame(pd.DataFrame([[k] + v for k, v in rows.items()], columns=["summary"] + list(cols)))
+
+
+def print_schema(fr, cols):
+    """`idf.select(cols).printSchema()` text."""
+    sdt = dict(fr.dtypes)
+    return "root\n" + "".join(" |-- %s: %s (nullable = true)\n" % (c, _PRINT_TYPE.get(sdt[c], sdt[c])) for c in cols)
+
+
+def _unique_over(fr, cols, cardinality_threshold, stats_unique):
+    """Columns whose unique count exceeds the threshold, from the code counts or a saved uniqueCount table."""
+    if stats_unique == {}:
+        present, _ = _present(fr, cols)
+        return [c for c in cols if len(present[c]) > cardinality_threshold]
+    from ..data_analyzer.quality_checker import _read_stats
+    df = _read_stats(stats_unique, ["attribute", "unique_values"])
+    return [a for a, u in zip(df["attribute"].tolist(), df["unique_values"].tolist()) if float(u) > cardinality_threshold]
+
+
+def cat_to_num_unsupervised(spark, idf, list_of_cols="all", drop_cols=[], method_type="label_encoding",
+                            index_order="frequencyDesc", cardinality_threshold=50, pre_existing_model=False,
+                            model_path="NA", stats_unique={}, output_mode="replace", print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:506-773, Spark 3): StringIndexer labels
+    (handleInvalid="keep") as an int column that keeps the source's nulls, or OneHotEncoder (keep, dropLast) as n + 1
+    dense int columns `<c>_0 .. <c>_n` appended after all columns, where nulls and unseen categories set `<c>_n`."""
+    fr = as_frame(idf)
+    cat_cols = attributeType_segregation(fr)[1]
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        list_of_cols = cat_cols
+    list_of_cols, drop_cols = _split(list_of_cols), _split(drop_cols)
+    if any(x not in cat_cols for x in list_of_cols):
+        raise TypeError("Invalid input for Column(s)")
+    if method_type not in ("onehot_encoding", "label_encoding"):
+        raise TypeError("Invalid input for method_type")
+    if index_order not in _INDEX_ORDERS:
+        raise TypeError("Invalid input for Encoding Index Order")
+    if output_mode not in ("replace", "append"):
+        raise TypeError("Invalid input for output_mode")
+    wanted = [c for c in dict.fromkeys(list_of_cols)]
+    over = set(_unique_over(fr, wanted, cardinality_threshold, stats_unique))
+    skip = [c for c in wanted if c in over and c not in drop_cols]
+    if skip:
+        warnings.warn("Columns dropped from encoding due to high cardinality: " + ",".join(skip))
+    cols = [c for c in wanted if c not in drop_cols + skip]
+    if not cols:
+        warnings.warn("No Encoding Computation - No categorical column(s) to transform")
+        return fr
+
+    if pre_existing_model:
+        model = load_indexer_model(model_path)
+        for c in cols:
+            if c not in model:
+                raise ValueError("cannot resolve '%s_index' given input columns" % c)
+        labels = {c: list(model[c]) for c in cols}
+        if method_type == "onehot_encoding":
+            _read_json_part(os.path.join(model_path, "cat_to_num_unsupervised", "encoder", "metadata"))
+    else:
+        present, _ = _present(fr, cols)
+        labels = {c: string_indexer_labels(present[c], index_order) for c in cols}
+        if model_path != "NA":
+            save_indexer_model(model_path, cols, [labels[c] for c in cols], index_order)
+            if method_type == "onehot_encoding":
+                save_onehot_model(model_path, cols)
+
+    if method_type == "onehot_encoding":
+        odf = _per_chunk(fr, lambda f: _apply_onehot(f, cols, labels, output_mode))
+    else:
+        odf = _per_chunk(fr, lambda f: _apply_label(f, cols, labels, output_mode))
+    if print_impact:
+        if method_type == "label_encoding":
+            new_cols = cols if output_mode == "replace" else [c + "_index" for c in cols]
+            print("Before")
+            summary_count_min_max(fr, cols).show(3, False)
+            print("After")
+            summary_count_min_max(odf, new_cols).show(3, False)
+        else:
+            new_cols = ["%s_%d" % (c, j) for c in cols for j in range(len(labels[c]) + 1)]
+            print("Before")
+            print(print_schema(fr, cols))
+            print("After")
+            print(print_schema(odf, (cols if output_mode == "append" else []) + new_cols))
+        if skip:
+            print("Columns dropped from encoding due to high cardinality: " + ",".join(skip))
+    return odf
+
+
+def _csv_field(v):
+    """A field as Spark's CSV writer puts it: null -> empty, "" -> \"\", quotes where needed, `\\` escapes quotes."""
+    if v is None:
+        return ""
+    if v == "" or any(ch in v for ch in ',"\n\r\\'):
+        return '"' + v.replace("\\", "\\\\").replace('"', '\\"') + '"'
+    return v
+
+
+def _csv_rows(path):
+    """Rows of a CSV file written by Spark or by _csv_field: an unquoted empty field is None, a quoted one ""."""
+    rows = []
+    for line in open(path, encoding="utf-8").read().splitlines():
+        out, i = [], 0
+        while True:
+            if i < len(line) and line[i] == '"':
+                j, buf = i + 1, []
+                while j < len(line) and line[j] != '"':
+                    if line[j] == "\\" and j + 1 < len(line):
+                        j += 1
+                    buf.append(line[j])
+                    j += 1
+                out.append("".join(buf))
+                i = j + 1
+            else:
+                j = line.find(",", i)
+                j = len(line) if j < 0 else j
+                out.append(line[i:j] if j > i else None)
+                i = j
+            if i >= len(line):
+                break
+            i += 1                                   # the comma
+            if i == len(line):
+                out.append(None)
+                break
+        rows.append(out)
+    return rows
+
+
+def _write_csv_dir(d, header, rows):
+    _clear_dir(d)
+    with open(os.path.join(d, "part-00000-c000.csv"), "w", encoding="utf-8") as f:
+        f.write(",".join(header) + "\n")
+        for r in rows:
+            f.write(",".join(_csv_field(v) for v in r) + "\n")
+    open(os.path.join(d, "_SUCCESS"), "w").close()
+
+
+def _read_csv_dir(d):
+    rows = []
+    for fn in _spark_parts(d):
+        if fn.endswith(".csv"):
+            rows += _csv_rows(fn)[1:]
+    return rows
+
+
+def save_supervised_model(model_path, col, table):
+    """<model_path>/cat_to_num_supervised/<col>/part-*.csv, header `<col>,<col>_encoded`: keys verbatim (null -> empty
+    field), values as java.lang.Double.toString."""
+    from ..shared.utils import jvm_double_str
+    _write_csv_dir(os.path.join(model_path, "cat_to_num_supervised", col), [col, col + "_encoded"],
+                   [[k, jvm_double_str(v)] for k, v in table])
+
+
+def load_supervised_model(model_path, col):
+    """-> [(key | None, value | None)] of a saved supervised model, keys read as strings."""
+    return [(r[0], None if len(r) < 2 or r[1] is None else float(r[1]))
+            for r in _read_csv_dir(os.path.join(model_path, "cat_to_num_supervised", col))]
+
+
+def _class_counts(fr, cols, label_col, event_label):
+    """-> ({col: all counts [size + 1]}, {col: event counts [size + 1]}, event rows, rows); slot 0 = the null group.  The
+    event class is label == event_label; every other row, a null label included, is class "0"."""
+    from ..shared.label_classes import label_bitmaps, masked
+    allc = profile.code_counts(fr, cols)
+    if getattr(fr, "is_partitioned", False):
+        n_event = sum(label_bitmaps(ch, label_col, event_label)[2] for ch in fr.chunks([label_col]))
+        if fr.group is not None:                     # row slabs on several ranks: the counts below are all-reduced
+            n_event = int(fr.group.all_reduce(np.array([n_event], np.int64))[0])
+        view = fr.map_chunks(fr._schema.select(cols), lambda ch: masked(ch, cols, label_bitmaps(ch, label_col, event_label)[0]))
+    else:
+        ev_w, _, n_event = label_bitmaps(fr, label_col, event_label)
+        view = masked(fr, cols, ev_w)
+    ev = {}
+    for c, h in zip(cols, engine.code_counts(view, cols)):
+        h = np.asarray(h, np.int64).copy()
+        h[0] = n_event - int(h[1:].sum())            # slot 0 of the masked pass mixes null and non-event rows
+        ev[c] = h
+    return {c: np.asarray(allc[c], np.int64) for c in cols}, ev, n_event, fr.n_rows
+
+
+def _supervised_table(fr, c, allc, ev):
+    """The reference's pivot: [(category | None, round(c1 / (c1 + c0), 4))] over the groups with rows."""
+    from ..shared.utils import spark_round
+    dic = fr.column(c).dictionary
+    out = [(None, spark_round(ev[0] / allc[0], 4))] if allc[0] else []
+    order = sorted((k for k in range(len(dic)) if allc[k + 1]), key=lambda k: _utf8(dic[k]))
+    return out + [(dic[k], spark_round(ev[k + 1] / allc[k + 1], 4)) for k in order]
+
+
+def _rate_table(dictionary, model):
+    """code_map table (float64) and entry validity of a supervised model: more than one row joins on the key (null rows
+    and keys the model lacks become null); exactly one row is a cross join (every row gets it, nulls included)."""
+    n = len(dictionary)
+    if len(model) == 1:
+        v = model[0][1]
+        return np.full(n + 1, 0.0 if v is None else v, np.float64), np.full(n + 1, v is not None)
+    m = {k: v for k, v in model if k is not None}
+    vals = [m.get(s) for s in dictionary] + [None]
+    return np.array([0.0 if v is None else v for v in vals], np.float64), np.array([v is not None for v in vals])
+
+
+def _apply_rates(fr, cols, models, output_mode):
+    tabs = [_rate_table(fr.column(c).dictionary, models[c]) for c in cols]
+    data, valid, nulls = engine.code_map(fr, cols, [t for t, _ in tabs], [v for _, v in tabs])
+    made = OrderedDict()
+    for c, d, v, nc in zip(cols, data, valid, nulls):
+        name = c if output_mode == "replace" else c + "_encoded"
+        made[name] = Column(name, "double", fr.n_rows, dev=d, dev_valid=v, anv_dtype=_lib.ANV_F64, null_count=int(nc))
+    new = OrderedDict((n, made[n] if n in made else fr.column(n)) for n in fr.columns)
+    for n, col in made.items():
+        new.setdefault(n, col)
+    return ColumnFrame(new, fr.n_rows)
+
+
+def cat_to_num_supervised(spark, idf, list_of_cols="all", drop_cols=[], label_col="label", event_label=1,
+                          pre_existing_model=False, model_path="NA", output_mode="replace", persist=False,
+                          persist_option=None, print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:776-962): each category becomes its
+    event rate round(c1 / (c1 + c0), 4) as a double column.  `persist` / `persist_option` are accepted and have nothing
+    to do on a resident frame.  model_path="NA" keeps the table in memory instead of round-tripping it through
+    `intermediate_data/`."""
+    fr = as_frame(idf)
+    cat_cols = attributeType_segregation(fr)[1]
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        list_of_cols = cat_cols
+    list_of_cols, drop_cols = _split(list_of_cols), _split(drop_cols)
+    cols = [e for e in dict.fromkeys(list_of_cols) if e not in drop_cols and e != label_col]
+    if any(x not in cat_cols for x in cols):
+        raise TypeError("Invalid input for Column(s)")
+    if not cols:
+        warnings.warn("No Categorical Encoding - No categorical column(s) to transform")
+        return fr
+    if label_col not in fr.columns:
+        raise TypeError("Invalid input for Label Column")
+
+    if pre_existing_model:
+        path = model_path if model_path != "NA" else "intermediate_data"
+        models = {c: load_supervised_model(path, c) for c in cols}
+    else:
+        allc, ev, n_event, n_rows = _class_counts(fr, cols, label_col, event_label)
+        if n_event == 0 or n_event == n_rows:
+            raise ValueError("cannot resolve '%s' given input columns: the label has no %s rows"
+                             % ("1" if n_event == 0 else "0", "event" if n_event == 0 else "non-event"))
+        models = {c: _supervised_table(fr, c, allc[c], ev[c]) for c in cols}
+        if model_path != "NA":
+            for c in cols:
+                save_supervised_model(model_path, c, models[c])
+    odf = _per_chunk(fr, lambda f: _apply_rates(f, cols, models, output_mode))
+    if print_impact:
+        out_cols = cols if output_mode == "replace" else [c + "_encoded" for c in cols]
+        print("Before: ")
+        summary_count_min_max(fr, cols).show(3, False)
+        print("After: ")
+        summary_count_min_max(odf, out_cols).show(3, False)
+    return odf
+
+
+def outlier_kept(counts, coverage, max_category):
+    """The categories outlier_categories keeps of [(category, count)] (non-null): in count-descending order (ties in UTF-8
+    order), with count_pct = count / total, rank = Spark's rank(), cumu = the running sum of count_pct and lag_cumu the
+    previous cumu (0 for the first), keep where not (cumu >= coverage and lag_cumu >= coverage) and rank <= max - 1."""
+    items = sorted(counts, key=lambda t: (-t[1], _utf8(t[0])))
+    total = float(sum(n for _, n in items))
+    kept, cumu, rank, prev = [], 0.0, 0, None
+    for i, (k, n) in enumerate(items):
+        if n != prev:
+            rank, prev = i + 1, n
+        lag = cumu
+        cumu += n / total
+        if not (cumu >= coverage and lag >= coverage) and rank <= max_category - 1:
+            kept.append(k)
+    return kept
+
+
+def save_outlier_model(model_path, params):
+    """<model_path>/outlier_categories/part-*.csv with `attribute,parameters` rows.  Spark's CSV writer trims leading and
+    trailing whitespace by default, so the saved categories are trimmed."""
+    _write_csv_dir(os.path.join(model_path, "outlier_categories"), ["attribute", "parameters"],
+                   [[c, k.strip()] for c, ks in params for k in ks])
+
+
+def load_outlier_model(model_path):
+    out = {}
+    for r in _read_csv_dir(os.path.join(model_path, "outlier_categories")):
+        if r and r[0] is not None:
+            out.setdefault(r[0], []).append(r[1] if len(r) > 1 else None)
+    return out
+
+
+def _outlier_map(dictionary, kept):
+    """-> (new dictionary: the kept categories and "outlier_categories" once, in UTF-8 order; int32 code table)."""
+    keep = set(kept)
+    new = sorted(set(s for s in dictionary if s in keep) | {_OUTLIER}, key=_utf8)
+    pos = {s: i for i, s in enumerate(new)}
+    return new, np.array([pos[s] if s in keep else pos[_OUTLIER] for s in dictionary] + [0], np.int32)
+
+
+def _apply_outliers(fr, cols, params, output_mode):
+    maps = [_outlier_map(fr.column(c).dictionary, params.get(c) or []) for c in cols]
+    data, _, _ = engine.code_map(fr, cols, [t for _, t in maps], [None] * len(cols))
+    made = OrderedDict()
+    for c, d, (dic, _) in zip(cols, data, maps):
+        src = fr.column(c)
+        name = c if output_mode == "replace" else c + "_outliered"
+        made[name] = Column(name, "string", fr.n_rows, dev=d, dev_valid=src.device()[1], anv_dtype=_lib.ANV_I32,
+                            null_count=src.null_count, dictionary=dic)
+    new = OrderedDict((n, made[n] if n in made else fr.column(n)) for n in fr.columns)
+    for n, col in made.items():
+        new.setdefault(n, col)
+    return ColumnFrame(new, fr.n_rows)
+
+
+def outlier_categories(spark, idf, list_of_cols="all", drop_cols=[], coverage=1.0, max_category=50,
+                       pre_existing_model=False, model_path="NA", output_mode="replace", print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:3489-3671): the less frequent
+    categories of each column become "outlier_categories"; nulls stay null."""
+    fr = as_frame(idf)
+    cat_cols = attributeType_segregation(fr)[1]
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        list_of_cols = cat_cols
+    list_of_cols, drop_cols = _split(list_of_cols), _split(drop_cols)
+    cols = [e for e in dict.fromkeys(list_of_cols) if e not in drop_cols]
+    if any(x not in cat_cols for x in cols):
+        raise TypeError("Invalid input for Column(s)")
+    if not cols:
+        warnings.warn("No Outlier Categories Computation - No categorical column(s) to transform")
+        return fr
+    if (coverage <= 0) | (coverage > 1):
+        raise TypeError("Invalid input for Coverage Value")
+    if max_category < 2:
+        raise TypeError("Invalid input for Maximum No. of Categories Allowed")
+    if output_mode not in ("replace", "append"):
+        raise TypeError("Invalid input for output_mode")
+
+    if pre_existing_model:
+        params = load_outlier_model(model_path)
+    else:
+        present, _ = _present(fr, cols)
+        params = OrderedDict((c, outlier_kept(present[c], coverage, max_category)) for c in cols)
+    odf = _per_chunk(fr, lambda f: _apply_outliers(f, cols, params, output_mode))
+    if not pre_existing_model and model_path != "NA":
+        save_outlier_model(model_path, params.items())
+    if print_impact:
+        from ..data_analyzer.stats_generator import uniqueCount_computation
+        out_cols = cols if output_mode == "replace" else [c + "_outliered" for c in cols]
+        before = uniqueCount_computation(spark, fr, cols).toPandas().rename(columns={"unique_values": "uniqueValues_before"})
+        after = uniqueCount_computation(spark, odf, out_cols).toPandas().rename(columns={"unique_values": "uniqueValues_after"})
+        from ..result import ResultFrame
+        ResultFrame(before).show(len(cols), False)
+        ResultFrame(after).show(len(cols), False)
+    return odf
+
+
+def cat_to_num_transformer(spark, idf, list_of_cols, drop_cols, method_type, encoding, label_col, event_label):
+    """The reference's dispatcher (transformers.py:428-503), kept as written: it validates `list_of_cols` and then calls
+    the encoders with their defaults.  Supervised mode turns the label into an int 0 / 1 column; "unsupervised" with a
+    label column returns None."""
+    fr = as_frame(idf)
+    cat_cols = attributeType_segregation(fr)[1]
+    if len(cat_cols) > 0:
+        if isinstance(list_of_cols, str) and list_of_cols == "all":
+            list_of_cols = cat_cols
+        list_of_cols = _split(list_of_cols)
+        if any(x not in cat_cols for x in list_of_cols):
+            raise TypeError("Invalid input for Column(s)")
+        if method_type == "supervised" and label_col is not None:
+            odf = cat_to_num_supervised(spark, fr, label_col=label_col, event_label=event_label)
+            return _label_to_int(odf, label_col, event_label)
+        elif method_type == "unsupervised" and label_col is None:
+            return cat_to_num_unsupervised(spark, fr, method_type=encoding, index_order="frequencyDesc")
+        return None
+    return fr
+
+
+def _label_to_int(fr, label_col, event_label):
+    """`withColumn(label, when(label == event_label, 1).otherwise(0))` as an int column with no nulls."""
+    from ..shared.label_classes import label_bitmaps
+
+    def one(f):
+        import torch
+        ev_w, _, _ = label_bitmaps(f, label_col, event_label)
+        rows = torch.arange(f.n_rows, device=ev_w.device)
+        bit = ((ev_w[rows >> 5] >> (rows & 31).to(torch.int32)) & 1).to(torch.int32)
+        new = OrderedDict((n, f.column(n)) for n in f.columns)
+        new[label_col] = Column(label_col, "int", f.n_rows, dev=bit, anv_dtype=_lib.ANV_I32, null_count=0)
+        return ColumnFrame(new, f.n_rows)
+    return _per_chunk(fr, one)

@@ -903,3 +903,112 @@ def scale_columns(frame: ColumnFrame, names, specs):
     launch_count += 1
     valid = [words[i, :n_words] if f else None for i, f in enumerate(flagged)]
     return [t[:frame.n_rows] for t in outs], valid, _host(nulls).view(np.int64)[:len(names)].copy()
+
+
+# ---- categorical encoding ------------------------------------------------------------------------
+
+_CODE_MAP_SPEC_DT = np.dtype([("size", "<i4"), ("out_dtype", "<i4"), ("table", "<u8"), ("table_valid", "<u8"),
+                              ("out", "<u8"), ("out_valid", "<u8")])
+_ONE_HOT_SPEC_DT = np.dtype([("size", "<i4"), ("k", "<i4"), ("index", "<u8"), ("out", "<u8"), ("stride", "<i8")])
+
+
+def _tables_to_dev(arrays):
+    """Host arrays -> one device buffer holding each at a 16-byte aligned offset; -> (buffer, device address of each)."""
+    offs, pos = [], 0
+    for a in arrays:
+        offs.append(pos)
+        pos += (a.nbytes + 15) // 16 * 16
+    host = np.zeros(max(pos, 16), np.uint8)
+    for a, o in zip(arrays, offs):
+        host[o:o + a.nbytes] = np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+    dev = _to_dev(host)
+    return dev, [dev.data_ptr() + o for o in offs]
+
+
+def code_map(frame: ColumnFrame, names, tables, entry_valid):
+    """anv_code_map: tables = per name, a host array of len(dictionary) + 1 entries (int32 or float64; the last is the null
+    slot); entry_valid = per name, a bool array of the same length or None.
+    -> (list of CUDA tensors [n_rows] in the table's dtype, list of int32 bitmap tensors [ceil(n_rows/32)] for the names
+    with entry_valid and None for the others (which keep the source's validity), int64 ndarray of null counts)."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names, tables, entry_valid = list(names), list(tables), list(entry_valid)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: code_map(frame, names[lo:hi], tables[lo:hi], entry_valid[lo:hi]), len(names))
+    n_words = (frame.n_rows + 31) // 32
+    padded = max((frame.n_rows + 3) // 4 * 4, 4)
+    host, outs, valid = [], [], []
+    for n, t, ev in zip(names, tables, entry_valid):
+        col = frame.column(n)
+        size = len(col.dictionary) if col.dictionary is not None else -1
+        if col.anv_dtype != _lib.ANV_I32 or size < 0 or t.dtype not in (np.int32, np.float64) or len(t) != size + 1 \
+                or (ev is not None and len(ev) != size + 1):
+            raise ValueError("code_map: column %r needs a string column and a table of its dictionary size + 1" % n)
+        host.append(t)
+        if ev is not None:
+            host.append(np.packbits(np.asarray(ev, bool), bitorder="little"))
+        outs.append(torch.empty(padded, dtype=torch.int32 if t.dtype == np.int32 else torch.float64, device="cuda"))
+        valid.append(torch.zeros(max(n_words, 1), dtype=torch.int32, device="cuda") if ev is not None else None)
+    if not names or not frame.n_rows:
+        return [t[:frame.n_rows] for t in outs], [None if v is None else v[:n_words] for v in valid], \
+            np.zeros(len(names), np.int64)
+    buf, addr = _tables_to_dev(host)
+    sp = np.zeros(len(names), _CODE_MAP_SPEC_DT)
+    a = iter(addr)
+    for i, (n, t, ev) in enumerate(zip(names, tables, entry_valid)):
+        od = _lib.ANV_I32 if t.dtype == np.int32 else _lib.ANV_F64
+        sp[i] = (len(t) - 1, od, next(a), next(a) if ev is not None else 0, outs[i].data_ptr(),
+                 valid[i].data_ptr() if valid[i] is not None else 0)
+    nulls = _dev_bytes(len(names) * 8)
+    desc, keep = frame.descriptors(names)
+    nbytes = input_bytes(frame, names)
+    if timer is not None:
+        nbytes += sum(frame.n_rows * t.element_size() + (n_words * 4 if v is not None else 0) for t, v in zip(outs, valid))
+    dspecs = _to_dev(sp)                                # held until the launch is enqueued
+    _call(L.anv_code_map, "anv_code_map", desc.data_ptr(), dspecs.data_ptr(), nulls.data_ptr(), len(names), frame.n_rows,
+          _stream(), nbytes=nbytes)
+    launch_count += 1
+    return [t[:frame.n_rows] for t in outs], [None if v is None else v[:n_words] for v in valid], \
+        _host(nulls).view(np.int64)[:len(names)].copy()
+
+
+def one_hot_stride(n_rows):
+    """Elements between the output columns of one_hot: n_rows rounded up to a multiple of 4 (16-byte aligned columns)."""
+    return max((int(n_rows) + 3) // 4 * 4, 4)
+
+
+def one_hot(frame: ColumnFrame, names, indexes, ks):
+    """anv_one_hot: indexes = per name, a host int32 array of len(dictionary) + 1 entries (the last is the null slot) in
+    [0, k); ks = output columns per name.  -> list of int32 CUDA tensors [k, n_rows], row j = (index == j), each row a
+    16-byte aligned view of one [k, one_hot_stride(n_rows)] allocation."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names, indexes, ks = list(names), list(indexes), [int(k) for k in ks]
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: one_hot(frame, names[lo:hi], indexes[lo:hi], ks[lo:hi]), len(names))
+    stride = one_hot_stride(frame.n_rows)
+    outs = []
+    for n, ix, k in zip(names, indexes, ks):
+        col = frame.column(n)
+        size = len(col.dictionary) if col.dictionary is not None else -1
+        if col.anv_dtype != _lib.ANV_I32 or size < 0 or ix.dtype != np.int32 or len(ix) != size + 1 or k < 1:
+            raise ValueError("one_hot: column %r needs a string column, an int32 index of its dictionary size + 1 and k >= 1"
+                             % n)
+        outs.append(torch.empty((k, stride), dtype=torch.int32, device="cuda"))
+    if not names or not frame.n_rows:
+        return [o[:, :frame.n_rows] for o in outs]
+    buf, addr = _tables_to_dev(indexes)
+    sp = np.zeros(len(names), _ONE_HOT_SPEC_DT)
+    for i in range(len(names)):
+        sp[i] = (len(indexes[i]) - 1, ks[i], addr[i], outs[i].data_ptr(), stride)
+    desc, keep = frame.descriptors(names)
+    nbytes = input_bytes(frame, names)
+    if timer is not None:
+        nbytes += sum(frame.n_rows * 4 * k for k in ks)
+    dspecs = _to_dev(sp)
+    _call(L.anv_one_hot, "anv_one_hot", desc.data_ptr(), dspecs.data_ptr(), len(names), frame.n_rows, _stream(),
+          nbytes=nbytes)
+    launch_count += 1
+    return [o[:, :frame.n_rows] for o in outs]

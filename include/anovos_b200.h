@@ -309,6 +309,41 @@ typedef struct {
 int anv_scale_columns(const anv_column_t* cols, const anv_scale_spec_t* specs, void* const* out_ptrs, uint32_t* out_validity,
                       int64_t* null_counts, int n_cols, int64_t n_rows, void* stream);
 
+/* ---- categorical encoding (cat_to_num_unsupervised, cat_to_num_supervised, outlier_categories;
+ *      data_transformer/transformers.py:506-962, 3489-3671).  Inputs are ANV_I32 dictionary-code columns.  A row reads the
+ *      table slot  valid(r) ? min((uint32)code, size) : size  where size is the column's dictionary size, so the table has
+ *      size + 1 entries and the last is the one null rows read.  A code outside [0, size) (negative included) reads the
+ *      null slot: no code reads outside the table.
+ * anv_code_map: out[r] = table[slot] in spec.out_dtype (ANV_I32 or ANV_F64).  table_valid [dev] ceil((size+1)/32) words
+ * or NULL: with it, row r is null where its entry's bit is clear; out_valid [dev] ceil(n_rows/32) words then gets the
+ * output bitmap (bits past n_rows are 0), null rows are written as 0 and null_counts[c] counts them.  Without it no bitmap
+ * is written (the output keeps the source's validity) and null_counts[c] is 0.  null_counts [dev] n_cols int64 (zeroed by
+ * the library).  out [dev] 16-byte aligned with room for n_rows rounded up to a multiple of 4 elements.  A spec whose
+ * column is not ANV_I32, whose out_dtype is not one of the above or whose pointers are missing leaves its column
+ * unwritten.  specs [dev] n_cols. */
+typedef struct {
+  int32_t size;                /* dictionary size: codes 0 .. size-1 */
+  int32_t out_dtype;           /* ANV_I32 or ANV_F64 */
+  const void* table;           /* [dev] size + 1 entries of out_dtype */
+  const uint32_t* table_valid; /* [dev] per-entry validity bitmap, or NULL */
+  void* out;                   /* [dev] output column */
+  uint32_t* out_valid;         /* [dev] output bitmap (needed when table_valid is set) */
+} anv_code_map_spec_t;
+int anv_code_map(const anv_column_t* cols, const anv_code_map_spec_t* specs, int64_t* null_counts, int n_cols, int64_t n_rows,
+                 void* stream);
+/* anv_one_hot: out[j * stride + r] = (index[slot] == j) as dense int32 for 0 <= j < k (no bitmap; rows n_rows up to the
+ * next multiple of 4 are written as 0, rows past that up to stride are left unwritten).  index [dev] size + 1 int32 entries; an entry outside [0, k) sets no output.  stride >= n_rows and a
+ * multiple of 4, out [dev] k * stride int32, 16-byte aligned: every output column is a 16-byte aligned view.  A spec that
+ * breaks these rules leaves its outputs unwritten.  specs [dev] n_cols. */
+typedef struct {
+  int32_t size;          /* dictionary size */
+  int32_t k;             /* output columns */
+  const int32_t* index;  /* [dev] size + 1 entries */
+  int32_t* out;          /* [dev] k * stride int32 */
+  int64_t stride;        /* elements from one output column to the next */
+} anv_one_hot_spec_t;
+int anv_one_hot(const anv_column_t* cols, const anv_one_hot_spec_t* specs, int n_cols, int64_t n_rows, void* stream);
+
 /* ---- Spark's Bernoulli row sampler (the DEFAULT path of drift_detector.statistics: use_sampling=True ->
  *      data_sampling.py:122-149 `idf.sample(False, fraction, seed)` / `stat.sampleBy("merge", fractions, seed)`,
  *      drift_detector.py:187-211).  One partition per call: Spark seeds XORShiftRandom with seed + partitionIndex,
