@@ -51,6 +51,12 @@ SCALE_DIV, SCALE_AFFINE, SCALE_CONST = 0, 1, 2   # ANV_SCALE_* modes of the head
 SCALE_NAN_TO_NULL = 1                            # ANV_SCALE_NAN_TO_NULL
 
 
+# ANV_TF_* ops of the header
+(TF_LN, TF_LOG10, TF_LOG2, TF_EXP, TF_POW_BASE, TF_POW, TF_SQRT, TF_CBRT, TF_SIN, TF_COS, TF_TAN, TF_ASIN, TF_ACOS, TF_ATAN,
+ TF_RADIANS, TF_MUL_INV, TF_FLOOR, TF_CEIL, TF_FACTORIAL, TF_REMAINDER, TF_ROUND) = range(21)
+TF_MAKES_NULLS = (TF_LN, TF_LOG10, TF_LOG2, TF_MUL_INV, TF_FACTORIAL)
+
+
 class AnvError(RuntimeError):
     pass
 
@@ -92,6 +98,9 @@ _SIGNATURES = {
     "anv_impute_fill": (C.c_int, [_P, _P, _P, _I, _L, _P]),
     "anv_valid_not_nan": (C.c_int, [_P, _I, _L, _P, _P, _P]),
     "anv_scale_columns": (C.c_int, [_P, _P, _P, _P, _P, _I, _L, _P]),
+    "anv_transform_columns": (C.c_int, [_P, _P, _P, _P, _P, _I, _L, _P]),
+    "anv_ks_candidates_workspace_bytes": (_SZ, [_L]),
+    "anv_ks_candidates": (C.c_int, [_P, _I, _L, _L, _P, _I, _P, _P, _P, _SZ, _P]),
     "anv_code_map": (C.c_int, [_P, _P, _P, _I, _L, _P]),
     "anv_one_hot": (C.c_int, [_P, _P, _I, _L, _P]),
     "anv_spark_hash_seed": (C.c_uint64, [_L]),

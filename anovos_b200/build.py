@@ -10,7 +10,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libanovos_b200.so")
-SOURCES = ["capi.cu", "scan_host.cu", "scan_mom.cu", "scan_hist.cu", "scan_fused.cu", "scan_assign.cu", "drift.cu", "synth.cu", "select.cu", "hll.cu", "sort.cu", "sample.cu", "gk_host.cu", "rows.cu", "impute.cu", "scale.cu", "encode.cu"]
+SOURCES = ["capi.cu", "scan_host.cu", "scan_mom.cu", "scan_hist.cu", "scan_fused.cu", "scan_assign.cu", "drift.cu", "synth.cu", "select.cu", "hll.cu", "sort.cu", "sample.cu", "gk_host.cu", "rows.cu", "impute.cu", "scale.cu", "encode.cu", "transform.cu"]
+# transform.cu restates fdlibm, which specifies no fused multiply-add: its products and sums are rounded one by one
+EXTRA_FLAGS = {"transform.cu": ["-fmad=false"]}
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17"] + GENCODE + ["-lineinfo",
               "--expt-relaxed-constexpr", "--expt-extended-lambda", "-Xcompiler", "-fPIC,-O3",
@@ -51,7 +53,8 @@ def build_variant(tag, defines):
     for s in SOURCES:
         obj = os.path.join(vdir, s.replace(".cu", ".o"))
         objs.append(obj)
-        cmd = [_nvcc()] + [f for f in NVCC_FLAGS if f not in ("-Xptxas", "-v")] + ["-D" + d for d in defines] + \
+        cmd = [_nvcc()] + [f for f in NVCC_FLAGS if f not in ("-Xptxas", "-v")] + EXTRA_FLAGS.get(s, []) + \
+              ["-D" + d for d in defines] + \
               ["-c", os.path.join(CSRC, s), "-o", obj]
         procs.append(subprocess.Popen(cmd))
     if any(p.wait() != 0 for p in procs):
@@ -80,7 +83,7 @@ def build(force=False, verbose=False):
             extra = ['-DANV_SOURCE_HASH="%s"' % digest]
             stale = stale or digest != old_digest
         if stale:
-            cmd = [_nvcc()] + NVCC_FLAGS + extra + ["-c", src, "-o", obj]
+            cmd = [_nvcc()] + NVCC_FLAGS + EXTRA_FLAGS.get(s, []) + extra + ["-c", src, "-o", obj]
             log = open(obj + ".log", "w")
             procs.append((s, subprocess.Popen(cmd, stdout=log, stderr=subprocess.STDOUT), obj + ".log"))
     failed = False

@@ -851,6 +851,256 @@ def normalization(idf, list_of_cols="all", drop_cols=[], pre_existing_model=Fals
     return odf
 
 
+# ---- feature_transformation, boxcox_transformation (reference transformers.py:3171-3486) ------------------------------
+#
+# Every method is one streaming pass (anv_transform_columns) with the semantics of the Spark expression the reference
+# builds: StrictMath's fdlibm for log / exp / pow, Spark's result types and nulls, round as HALF_UP of the shortest
+# decimal.  Every op is row-local, so a partitioned frame transforms chunk by chunk.  Semantics and deviations: DESIGN.md
+# section 1.
+
+_TF_METHODS = ("ln", "log10", "log2", "exp", "powOf2", "powOf10", "powOfN", "sqrt", "cbrt", "sq", "cb", "toPowerN", "sin",
+               "cos", "tan", "asin", "acos", "atan", "radians", "remainderDivByN", "factorial", "mul_inv", "floor", "ceil",
+               "roundN")
+_TF_WITH_N = ("powOfN", "toPowerN", "remainderDivByN", "roundN")
+_TF_DOUBLE = {"ln": _lib.TF_LN, "log10": _lib.TF_LOG10, "log2": _lib.TF_LOG2, "exp": _lib.TF_EXP, "sqrt": _lib.TF_SQRT,
+              "cbrt": _lib.TF_CBRT, "sin": _lib.TF_SIN, "cos": _lib.TF_COS, "tan": _lib.TF_TAN, "asin": _lib.TF_ASIN,
+              "acos": _lib.TF_ACOS, "atan": _lib.TF_ATAN, "radians": _lib.TF_RADIANS, "mul_inv": _lib.TF_MUL_INV}
+_TF_POW = {"powOf2": (_lib.TF_POW_BASE, 2.0), "powOf10": (_lib.TF_POW_BASE, 10.0), "sq": (_lib.TF_POW, 2.0),
+           "cb": (_lib.TF_POW, 3.0)}
+_INT_RANK = {_lib.ANV_I32: 0, _lib.ANV_I64: 1, _lib.ANV_F32: 2, _lib.ANV_F64: 3}
+
+
+def _number(N, method_type):
+    if isinstance(N, bool) or not isinstance(N, (int, float)):
+        raise TypeError("N must be a number for method_type %s" % method_type)
+    return N
+
+
+def _literal_dtype(N):
+    """The type of F.lit(N): int in 32 bits -> int, other ints -> bigint, float -> double."""
+    if isinstance(N, float):
+        return _lib.ANV_F64
+    return _lib.ANV_I32 if -(1 << 31) <= N < (1 << 31) else _lib.ANV_I64
+
+
+def transform_spec(method_type, N, in_dtype):
+    """The anv_transform_columns spec (op, out dtype, n, a) of one column, or (None, out dtype) for a column that is all
+    null (x % 0, Spark's Remainder by zero)."""
+    if method_type in _TF_DOUBLE:
+        return (_TF_DOUBLE[method_type], _lib.ANV_F64, 0, 0.0)
+    if method_type in _TF_POW:
+        op, a = _TF_POW[method_type]
+        return (op, _lib.ANV_F64, 0, a)
+    if method_type in ("powOfN", "toPowerN"):
+        if N is None:                                   # F.pow(None, x) / x ** None: a null literal, an all-null column
+            return (None, _lib.ANV_F64)
+        return (_lib.TF_POW_BASE if method_type == "powOfN" else _lib.TF_POW, _lib.ANV_F64, 0, float(_number(N, method_type)))
+    if method_type in ("floor", "ceil", "factorial"):
+        op = {"floor": _lib.TF_FLOOR, "ceil": _lib.TF_CEIL, "factorial": _lib.TF_FACTORIAL}[method_type]
+        return (op, _lib.ANV_I64, 0, 0.0)
+    if method_type == "remainderDivByN":
+        if N is None:                                   # x % F.lit(None): null in the column's type
+            return (None, in_dtype)
+        N = _number(N, method_type)
+        lit = _literal_dtype(N)
+        od = in_dtype if _INT_RANK[in_dtype] >= _INT_RANK[lit] else lit
+        if N == 0:
+            return (None, od)
+        if od in (_lib.ANV_F32, _lib.ANV_F64):
+            a = float(np.float32(N)) if od == _lib.ANV_F32 else float(N)
+            return (_lib.TF_REMAINDER, od, 0, a)
+        return (_lib.TF_REMAINDER, od, int(N), 0.0)
+    # roundN: F.round(x, N) takes an int scale
+    if isinstance(N, bool) or not isinstance(N, int):
+        raise TypeError("N must be an integer for method_type roundN")
+    if in_dtype in (_lib.ANV_F32, _lib.ANV_F64) and not -22 <= N <= 22:
+        raise ValueError("roundN of a float or double column takes -22 <= N <= 22 on the device, got %d" % N)
+    return (_lib.TF_ROUND, in_dtype, int(N), 0.0)
+
+
+def _transform_cols(fr, list_of_cols, drop_cols):
+    """The reference's column checks: -> the numeric columns, first-seen order."""
+    num_cols = attributeType_segregation(fr)[0]
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        list_of_cols = num_cols
+    drop = _names(drop_cols)
+    cols = [c for c in dict.fromkeys(_names(list_of_cols)) if c not in drop]
+    if len(cols) == 0 or any(c not in num_cols for c in cols):
+        raise TypeError("Invalid input for Column(s)")
+    sdt = dict(fr.dtypes)
+    for c in cols:
+        if sdt[c] not in _ANV_OF_SDTYPE:
+            raise TypeError("transformation of %s column %r is not supported on the device" % (sdt[c], c))
+    return cols
+
+
+def _apply_transform(fr, cols, specs, out_names):
+    """Write op(col) for each (col, spec) under its output name -> new frame: a name that exists keeps its position (the
+    reference's withColumn), a new one goes after all existing columns, in list order."""
+    torch = None
+    run = [i for i, s in enumerate(specs) if s[0] is not None]
+    data, valid, nulls = engine.transform_columns(fr, [cols[i] for i in run], [specs[i] for i in run])
+    made = {}
+    for k, i in enumerate(run):
+        src = fr.column(cols[i])
+        od = specs[i][1]
+        if valid[k] is not None:
+            v, nc = valid[k], int(nulls[k])
+        else:
+            v, nc = src.device()[1], src.null_count
+        made[out_names[i]] = Column(out_names[i], _SDTYPE_OF_ANV[od], fr.n_rows, dev=data[k], dev_valid=v, anv_dtype=od,
+                                    null_count=nc)
+    for i, s in enumerate(specs):
+        if s[0] is None:
+            torch = torch or _lib.require_cuda()
+            d, _ = fr.column(cols[i]).device()
+            od = s[1]
+            made[out_names[i]] = Column(out_names[i], _SDTYPE_OF_ANV[od], fr.n_rows,
+                                        dev=torch.zeros(max(fr.n_rows, 1), dtype=getattr(torch, engine._TORCH_OF_ANV[od]),
+                                                        device=d.device)[:fr.n_rows],
+                                        dev_valid=torch.zeros(max((fr.n_rows + 31) // 32, 1), dtype=torch.int32,
+                                                              device=d.device),
+                                        anv_dtype=od, null_count=fr.n_rows)
+    new = OrderedDict()
+    for n in fr.columns:
+        new[n] = made.pop(n) if n in made else fr.column(n)
+    for n in out_names:
+        if n in made:
+            new[n] = made.pop(n)
+    return ColumnFrame(new, fr.n_rows)
+
+
+def _transformed_frame(fr, cols, specs, out_names):
+    if getattr(fr, "is_partitioned", False):
+        schema = _apply_transform(fr._schema, cols, specs, out_names)
+        return fr.map_chunks(schema, lambda ch: _apply_transform(ch, cols, specs, out_names))
+    return _apply_transform(fr, cols, specs, out_names)
+
+
+def feature_transformation(idf, list_of_cols="all", drop_cols=[], method_type="sqrt", N=None, output_mode="replace",
+                           print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:3171-3324): one of 25 row-wise maths
+    transforms, with Spark's result types and nulls."""
+    fr = as_frame(idf)
+    cols = _transform_cols(fr, list_of_cols, drop_cols)
+    if method_type not in _TF_METHODS:
+        raise TypeError("Invalid input method_type")
+    sdt = dict(fr.dtypes)
+    specs = [transform_spec(method_type, N, _ANV_OF_SDTYPE[sdt[c]]) for c in cols]
+    if output_mode == "replace":
+        out_names = list(cols)
+    elif method_type in _TF_WITH_N:
+        out_names = [c + "_" + method_type[:-1] + str(N) for c in cols]
+    else:
+        out_names = [c + "_" + method_type for c in cols]
+    odf = _transformed_frame(fr, cols, specs, out_names)
+    if print_impact:
+        print("Before:")
+        describe(fr, cols).show(5, False)
+        print("After:")
+        describe(odf, out_names).show(5, False)
+    return odf
+
+
+BOXCOX_LAMBDAS = (1, -1, 0.5, -0.5, 2, -2, 0.25, -0.25, 3, -3, 4, -4, 5, -5)
+
+
+def ks_statistics(fr, c):
+    """The Kolmogorov-Smirnov statistic against N(0, 1) of pow(c, lambda) for each BOXCOX_LAMBDAS and of log(c), over all
+    rows with null rows as the value 0 (recalled from PySpark: `rdd.flatMap` hands None to the JVM, which unboxes it as
+    0.0).  One sort and one candidate pass on the device (anv_ks_candidates); the run of zeros adds one term here."""
+    n = fr.n_rows
+    n_null = n - int(profile.moments(fr, [c])[c]["n_valid"])
+    d, below = engine.ks_candidates(fr, c, BOXCOX_LAMBDAS, n_null)
+    if n_null:
+        for k in range(len(d)):
+            a = below if k == len(BOXCOX_LAMBDAS) else 0       # zeros sit after the log values below 0
+            d[k] = max(d[k], 0.5 - a / n, (a + n_null) / n - 0.5)
+    return d
+
+
+def boxcox_search(fr, cols):
+    """The reference's lambda search (transformers.py:3424-3443), its selection loop kept literally: per column the first
+    candidate with a strictly larger p-value wins, starting from 0; a column where none beats 0 keeps the previous
+    column's lambda, and the first column raises UnboundLocalError."""
+    from ..shared.ks import p_value
+    if getattr(fr, "is_partitioned", False):                 # the test needs each column whole
+        import pyarrow as pa
+        fr = as_frame(pa.concat_tables([ch.to_arrow().select(cols) for ch in fr.chunks(cols)]))
+    out, best = [], None
+    for c in cols:
+        d = ks_statistics(fr, c)
+        best_p = 0
+        for lam, dk in zip(list(BOXCOX_LAMBDAS) + [0], d):
+            p = p_value(float(dk), fr.n_rows)
+            if p > best_p:
+                best_p, best = p, lam
+        if best is None:
+            raise UnboundLocalError("cannot access local variable 'best_lambdaVal' where it is not associated with a value")
+        out.append(best)
+    return out
+
+
+def skewness_row(fr, cols):
+    """`F.skewness` of each column from the moments pass: sqrt(n) * m3 / sqrt(m2^3), null for n = 0 or m2 = 0."""
+    from ..shared.utils import jvm_double_str
+    mom = profile.moments(fr, cols)
+    out = []
+    for c in cols:
+        n, m2, m3 = int(mom[c]["n_valid"]), float(mom[c]["m2"]), float(mom[c]["m3"])
+        out.append("null" if n == 0 or m2 == 0 else jvm_double_str(math.sqrt(n) * m3 / math.sqrt(m2 * m2 * m2)))
+    return out
+
+
+def _describe_skew(fr, cols):
+    import pandas as pd
+    from ..result import ResultFrame
+    d = describe(fr, cols).toPandas()
+    d = pd.concat([d, pd.DataFrame([["skewness"] + skewness_row(fr, cols)], columns=d.columns)], ignore_index=True)
+    return ResultFrame(d)
+
+
+def boxcox_transformation(idf, list_of_cols="all", drop_cols=[], boxcox_lambda=None, output_mode="replace",
+                          print_impact=False):
+    """Same arguments, errors and returned frame as the reference (transformers.py:3327-3486): pow(x, lambda), or log(x)
+    for lambda 0; lambda 1 leaves the column as it is.  boxcox_lambda=None picks each column's lambda by the reference's
+    Kolmogorov-Smirnov search (boxcox_search)."""
+    fr = as_frame(idf)
+    cols = _transform_cols(fr, list_of_cols, drop_cols)
+    mom = profile.moments(fr, cols)
+    mins = [float(mom[c]["min"]) if int(mom[c]["n_valid"]) else None for c in cols]
+    if any(m is None for m in mins):
+        raise TypeError("'<=' not supported between instances of 'NoneType' and 'int'")
+    if any(m <= 0 for m in mins):
+        print(" ".join("min(%s)=%r" % (c, m) for c, m in zip(cols, mins)))
+        raise ValueError("Data must be positive")
+    if boxcox_lambda is None:
+        lambdas = boxcox_search(fr, cols)
+    elif isinstance(boxcox_lambda, (list, tuple)):
+        if len(boxcox_lambda) != len(cols) or not all(isinstance(v, (float, int)) for v in boxcox_lambda):
+            raise TypeError("Invalid input for boxcox_lambda")
+        lambdas = list(boxcox_lambda)
+    elif isinstance(boxcox_lambda, (float, int)):
+        lambdas = [boxcox_lambda] * len(cols)
+    else:
+        raise TypeError("Invalid input for boxcox_lambda")
+    run = [(c, lam) for c, lam in zip(cols, lambdas) if lam != 1]
+    if not run:
+        warnings.warn("lambdaVal for all columns are 1 so no transformation is performed and idf is returned")
+        return idf
+    specs = [(_lib.TF_LN, _lib.ANV_F64, 0, 0.0) if lam == 0 else (_lib.TF_POW, _lib.ANV_F64, 0, float(lam)) for _, lam in run]
+    out_names = [c + "_bxcx_" + str(lam) if output_mode == "append" else c for c, lam in run]
+    odf = _transformed_frame(fr, [c for c, _ in run], specs, out_names)
+    if print_impact:
+        print("Transformed Columns: ", cols)
+        print("Best BoxCox Parameter(s): ", lambdas)
+        print("Before:")
+        _describe_skew(fr, cols).show(6, False)
+        print("After:")
+        _describe_skew(odf, cols if output_mode == "replace" else out_names).show(6, False)
+    return odf
+
+
 # ---- categorical encoding: cat_to_num_unsupervised, cat_to_num_supervised, outlier_categories ------------------------
 # (reference transformers.py:428-962, 3489-3671)
 #

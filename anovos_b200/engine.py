@@ -905,6 +905,82 @@ def scale_columns(frame: ColumnFrame, names, specs):
     return [t[:frame.n_rows] for t in outs], valid, _host(nulls).view(np.int64)[:len(names)].copy()
 
 
+# ---- feature transformation ----------------------------------------------------------------------
+
+_TRANSFORM_SPEC_DT = np.dtype([("op", "<i4"), ("out_dtype", "<i4"), ("n", "<i8"), ("a", "<f8")])
+_FLOATS = (_lib.ANV_F32, _lib.ANV_F64)
+
+
+def transform_spec_ok(op, in_dtype, out_dtype, n):
+    """The (op, input, output) combinations of the header's ANV_TF_* table."""
+    if op in (_lib.TF_FLOOR, _lib.TF_CEIL, _lib.TF_FACTORIAL):
+        return out_dtype == _lib.ANV_I64
+    if op == _lib.TF_REMAINDER:
+        return {_lib.ANV_F64: True, _lib.ANV_F32: in_dtype == _lib.ANV_F32, _lib.ANV_I32: in_dtype == _lib.ANV_I32 and n != 0,
+                _lib.ANV_I64: in_dtype in (_lib.ANV_I32, _lib.ANV_I64) and n != 0}.get(out_dtype, False)
+    if op == _lib.TF_ROUND:
+        return out_dtype == in_dtype and (in_dtype not in _FLOATS or -22 <= n <= 22)
+    return _lib.TF_LN <= op <= _lib.TF_MUL_INV and out_dtype == _lib.ANV_F64
+
+
+def transform_columns(frame: ColumnFrame, names, specs):
+    """anv_transform_columns: specs = one (op, out anv dtype, n, a) per name (_lib.TF_*).
+    -> (list of CUDA tensors [n_rows] in the output dtype, list of int32 bitmap tensors [ceil(n_rows/32)] for the ops that
+    make nulls (_lib.TF_MAKES_NULLS) and None for the others (which keep the source's validity), int64 ndarray of null
+    counts)."""
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names, specs = list(names), list(specs)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: transform_columns(frame, names[lo:hi], specs[lo:hi]), len(names))
+    sp = np.zeros(len(names), _TRANSFORM_SPEC_DT)
+    outs, ptrs = [], np.zeros(len(names), np.uint64)
+    padded = (frame.n_rows + 3) // 4 * 4
+    for i, (n, (op, od, k, a)) in enumerate(zip(names, specs)):
+        ind = frame.column(n).anv_dtype
+        if ind not in _NP_OF_ANV or not transform_spec_ok(op, ind, od, k):
+            raise ValueError("transform_columns: column %r: no op %r from dtype %r to %r with n = %r" % (n, op, ind, od, k))
+        sp[i] = (op, od, k, a)
+        t = torch.empty(max(padded, 4), dtype=getattr(torch, _TORCH_OF_ANV[od]), device="cuda")
+        outs.append(t)
+        ptrs[i] = t.data_ptr()
+    n_words = (frame.n_rows + 31) // 32
+    flagged = [s[0] in _lib.TF_MAKES_NULLS for s in specs]
+    valid = [torch.zeros(max(n_words, 1), dtype=torch.int32, device="cuda")[:n_words] if f else None for f in flagged]
+    vptrs = np.array([0 if v is None else v.data_ptr() for v in valid], np.uint64)
+    if not names or not frame.n_rows:
+        return [t[:frame.n_rows] for t in outs], valid, np.zeros(len(names), np.int64)
+    nulls = _dev_bytes(len(names) * 8)
+    desc, keep = frame.descriptors(names)
+    nbytes = input_bytes(frame, names)
+    if timer is not None:
+        nbytes += sum(frame.n_rows * t.element_size() + (n_words * 4 if f else 0) for t, f in zip(outs, flagged))
+    dspecs, dptrs = _to_dev(sp), _to_dev(ptrs)          # held until the launch is enqueued
+    dvptrs = _to_dev(vptrs) if any(flagged) else None
+    _call(L.anv_transform_columns, "anv_transform_columns", desc.data_ptr(), dspecs.data_ptr(), dptrs.data_ptr(),
+          None if dvptrs is None else dvptrs.data_ptr(), nulls.data_ptr(), len(names), frame.n_rows, _stream(), nbytes=nbytes)
+    launch_count += 1
+    return [t[:frame.n_rows] for t in outs], valid, _host(nulls).view(np.int64)[:len(names)].copy()
+
+
+def ks_candidates(frame: ColumnFrame, name, lambdas, n_null):
+    """anv_ks_candidates on one column (values > 0 where valid, n_null null rows): -> (float64 ndarray of len(lambdas) + 1 statistics over the
+    valid rows, for pow(x, lambda) then log(x); the count of valid values below 1)."""
+    global launch_count
+    _lib.require_cuda()
+    L = _lib.lib()
+    n = frame.n_rows
+    desc, keep = frame.descriptors([name])
+    lam = (C.c_double * max(len(lambdas), 1))(*[float(v) for v in lambdas])
+    d_out, below = _dev_bytes(8 * (len(lambdas) + 1)), _dev_bytes(8)
+    ws = _dev_bytes(L.anv_ks_candidates_workspace_bytes(n))
+    _call(L.anv_ks_candidates, "anv_ks_candidates", desc.data_ptr(), 0, n, int(n_null), lam, len(lambdas),
+          d_out.data_ptr(), below.data_ptr(), ws.data_ptr(), ws.numel(), _stream(), nbytes=input_bytes(frame, [name]))
+    launch_count += 1
+    return _host(d_out).view(np.float64)[:len(lambdas) + 1].copy(), int(_host(below).view(np.int64)[0])
+
+
 # ---- categorical encoding ------------------------------------------------------------------------
 
 _CODE_MAP_SPEC_DT = np.dtype([("size", "<i4"), ("out_dtype", "<i4"), ("table", "<u8"), ("table_valid", "<u8"),

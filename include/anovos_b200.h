@@ -309,6 +309,73 @@ typedef struct {
 int anv_scale_columns(const anv_column_t* cols, const anv_scale_spec_t* specs, void* const* out_ptrs, uint32_t* out_validity,
                       int64_t* null_counts, int n_cols, int64_t n_rows, void* stream);
 
+/* ---- feature transformation (feature_transformation, boxcox_transformation; data_transformer/transformers.py:3171-3486).
+ * anv_transform_columns: one streaming pass per column writes out[r] = op(x) for every row r, with Spark's semantics of
+ * the expression the reference builds.  x is converted to double (a bigint beyond 2^53 rounds to nearest) except where an
+ * op names integer arithmetic.  Every double operation is rounded on its own (no FMA contraction).
+ *   LN, LOG10, LOG2     StrictMath.log / log10 (fdlibm 5.3); LOG2 = log(x) / log(2).  x <= 0 -> null.       out F64
+ *   EXP                 StrictMath.exp                                                                       out F64
+ *   POW_BASE            StrictMath.pow(a, x)   (powOf2, powOf10, powOfN)                                     out F64
+ *   POW                 StrictMath.pow(x, a)   (sq, cb, toPowerN, Box-Cox)                                   out F64
+ *   SQRT                correctly rounded square root                                                        out F64
+ *   CBRT, SIN, COS, TAN, ASIN, ACOS, ATAN   CUDA's double functions (within 2 ulp)                           out F64
+ *   RADIANS             x * 0.017453292519943295                                                             out F64
+ *   MUL_INV             1 / x; x == 0 -> null                                                                out F64
+ *   FLOOR, CEIL         floor / ceil then Double.toLong (NaN -> 0, saturating); integer x: itself            out I64
+ *   FACTORIAL           x cast to int (float: truncated, saturating, NaN -> 0; bigint: low 32 bits), then n!;
+ *                       outside 0..20 -> null                                                                out I64
+ *   REMAINDER           Java's x % N in out_dtype: floating outputs fmod(x, a) (a is N in that type), integer
+ *                       outputs the truncated remainder by n (n != 0; x % -1 = 0)     out F32 (F32 x), F64, I32 (I32 x), I64
+ *   ROUND               BigDecimal(Double.toString(x)).setScale(n, HALF_UP) back in x's type; floating x needs
+ *                       -22 <= n <= 22; integer x: unchanged for n >= 0, HALF_UP in integer arithmetic (wrapping
+ *                       to the type, as BigDecimal.intValue / longValue do) for n < 0                       out = x's type
+ * Only LN, LOG10, LOG2, MUL_INV and FACTORIAL make nulls: for them out_valid_ptrs[c] ([dev] ceil(n_rows/32) words) gets
+ * the output bitmap (source valid and op defined; bits past n_rows are 0); the other ops write no bitmap (the output keeps the
+ * source's validity).  Null rows are written as 0.  null_counts [dev] n_cols int64 (zeroed by the library): the null
+ * rows of each output.  A spec whose op or out_dtype does not fit the table leaves its column unwritten.
+ * specs [dev] n_cols; out_ptrs [dev] n_cols device pointers, each 16-byte aligned with room for n_rows rounded up to a
+ * multiple of 4 elements; out_valid_ptrs [dev] n_cols bitmap pointers (NULL entries for the ops that make no nulls), or
+ * NULL when no spec makes nulls. */
+#define ANV_TF_LN 0
+#define ANV_TF_LOG10 1
+#define ANV_TF_LOG2 2
+#define ANV_TF_EXP 3
+#define ANV_TF_POW_BASE 4
+#define ANV_TF_POW 5
+#define ANV_TF_SQRT 6
+#define ANV_TF_CBRT 7
+#define ANV_TF_SIN 8
+#define ANV_TF_COS 9
+#define ANV_TF_TAN 10
+#define ANV_TF_ASIN 11
+#define ANV_TF_ACOS 12
+#define ANV_TF_ATAN 13
+#define ANV_TF_RADIANS 14
+#define ANV_TF_MUL_INV 15
+#define ANV_TF_FLOOR 16
+#define ANV_TF_CEIL 17
+#define ANV_TF_FACTORIAL 18
+#define ANV_TF_REMAINDER 19
+#define ANV_TF_ROUND 20
+typedef struct {
+  int32_t op;        /* ANV_TF_* */
+  int32_t out_dtype; /* see the table */
+  int64_t n;         /* integer parameter: REMAINDER on integer outputs, ROUND */
+  double a;          /* double parameter: POW_BASE, POW, REMAINDER on floating outputs */
+} anv_transform_spec_t;
+int anv_transform_columns(const anv_column_t* cols, const anv_transform_spec_t* specs, void* const* out_ptrs,
+                          uint32_t* const* out_valid_ptrs, int64_t* null_counts, int n_cols, int64_t n_rows, void* stream);
+/* anv_ks_candidates: the Kolmogorov-Smirnov statistics of boxcox_transformation's lambda search for column c of cols
+ * [dev] (values > 0 where valid; n_null of its n_rows < 2^32 rows are null and enter every test as the value 0).  Sorts
+ * the column once, then d_out [dev] n_pow + 1 doubles gets, for y = StrictMath.pow(x, lambdas[k]) (k < n_pow, lambdas on
+ * the host, n_pow < 16) and y = StrictMath.log(x) (k = n_pow), the largest max(Phi(y) - (r-1)/n, r/n - Phi(y)) over the
+ * VALID rows (r: y's 1-based rank among all n rows, the zeros included; Phi the standard normal CDF, CUDA's erfc).  The
+ * zeros' own term is left to the caller; n_below_one [dev] 1 int64 gets the count of valid values below 1 (where the
+ * zeros fall among log(x)).  workspace: anv_ks_candidates_workspace_bytes(n_rows) bytes. */
+size_t anv_ks_candidates_workspace_bytes(int64_t n_rows);
+int anv_ks_candidates(const anv_column_t* cols, int c, int64_t n_rows, int64_t n_null, const double* lambdas, int n_pow,
+                      double* d_out, int64_t* n_below_one, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- categorical encoding (cat_to_num_unsupervised, cat_to_num_supervised, outlier_categories;
  *      data_transformer/transformers.py:506-962, 3489-3671).  Inputs are ANV_I32 dictionary-code columns.  A row reads the
  *      table slot  valid(r) ? min((uint32)code, size) : size  where size is the column's dictionary size, so the table has
