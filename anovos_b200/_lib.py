@@ -103,6 +103,8 @@ _SIGNATURES = {
     "anv_ks_candidates": (C.c_int, [_P, _I, _L, _L, _P, _I, _P, _P, _P, _SZ, _P]),
     "anv_code_map": (C.c_int, [_P, _P, _P, _I, _L, _P]),
     "anv_one_hot": (C.c_int, [_P, _P, _I, _L, _P]),
+    "anv_flag_members": (C.c_int, [_P, _P, _I, _L, _P]),
+    "anv_flag_members_smem_keys": (C.c_int, []),
     "anv_spark_hash_seed": (C.c_uint64, [_L]),
     "anv_spark_sample_mask": (C.c_int, [_L, _L, _P, _P, _I, _P, _P]),
     "anv_synth_f32": (C.c_int, [_P, _P, _L, C.c_uint64, C.c_uint32, _I, C.c_float, C.c_float, C.c_float, _P]),

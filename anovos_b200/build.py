@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libanovos_b200.so")
-SOURCES = ["capi.cu", "scan_host.cu", "scan_mom.cu", "scan_hist.cu", "scan_fused.cu", "scan_assign.cu", "drift.cu", "synth.cu", "select.cu", "hll.cu", "sort.cu", "sample.cu", "gk_host.cu", "rows.cu", "impute.cu", "scale.cu", "encode.cu", "transform.cu"]
+SOURCES = ["capi.cu", "scan_host.cu", "scan_mom.cu", "scan_hist.cu", "scan_fused.cu", "scan_assign.cu", "drift.cu", "synth.cu", "select.cu", "hll.cu", "sort.cu", "sample.cu", "gk_host.cu", "rows.cu", "impute.cu", "scale.cu", "encode.cu", "transform.cu", "invalid.cu"]
 # transform.cu restates fdlibm, which specifies no fused multiply-add: its products and sums are rounded one by one
 EXTRA_FLAGS = {"transform.cu": ["-fmad=false"]}
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -7,9 +7,11 @@ N2), same signatures and outputs as the reference
   outlier_detection     :550-1045
   IDness_detection      :1048-1182
   biasedness_detection  :1185-1339
+  invalidEntries_detection :1342-1711 (per-value rules on the host once per distinct value, one table-membership pass
+                        on the device that counts and nulls the flagged rows - csrc/invalid.cu)
 Each returns (odf, odf_print) where the reference does.  The per-row work (row null counts, distinct rows, null counts,
-distinct counts, modes, percentile / moment thresholds, the outlier compare pass) runs in the CUDA kernels.  Invalid-entry
-detection and the imputation treatments (MMM / KNN / regression / MF / auto) are not part of this build."""
+distinct counts, modes, percentile / moment thresholds, the outlier compare pass) runs in the CUDA kernels.  The imputation
+treatments KNN / regression / MF / auto are not part of this build."""
 from __future__ import annotations
 
 import math
@@ -606,3 +608,176 @@ def outlier_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_si
         out.show(len(rows))
         return odf, out
     return odf
+
+
+# ---- invalidEntries_detection --------------------------------------------------------------------------
+
+_INVALID_PRINT_COLS = ["attribute", "invalid_entries", "invalid_count", "invalid_pct"]
+
+
+def _distinct_numeric(fr, c):
+    """Distinct values of numeric column c over its valid rows (host array of its dtype, NaN payloads canonical): a sort
+    on the device of the raw bits, so -0.0 and 0.0 stay apart.  A row-partitioned frame unions its chunks'."""
+    from ..shared.invalid_rules import canonical_nan_bits
+    if getattr(fr, "is_partitioned", False):
+        if fr.group is not None:
+            raise NotImplementedError("invalidEntries_detection of float columns, or of integer columns in manual / both "
+                                      "mode, needs each column's distinct values on one rank; use "
+                                      "partitioned.repartition_to_columns first (auto mode on integer and string columns "
+                                      "works on row slabs)")
+        parts = [_distinct_numeric(ch, c) for ch in fr.chunks([c])]
+        return np.concatenate(parts) if parts else np.zeros(0, engine._NP_OF_ANV[fr.column(c).anv_dtype])
+    torch = _lib.require_cuda()
+    col = fr.column(c)
+    d, v = col.device()
+    d = d[:fr.n_rows]
+    if v is not None:
+        d = d[fr.valid_mask(c)]
+    if d.is_floating_point():
+        d = torch.where(torch.isnan(d), torch.full_like(d, float("nan")), d)
+        d = d.view(torch.int32 if d.element_size() == 4 else torch.int64)
+    host = torch.unique(d).cpu().numpy()
+    if col.anv_dtype in (_lib.ANV_F32, _lib.ANV_F64):
+        host = canonical_nan_bits(host.view(np.float32 if col.anv_dtype == _lib.ANV_F32 else np.float64))
+    return host
+
+
+def _invalid_table(fr, c, rule):
+    """-> (sorted table of the column's invalid values for engine.flag_members, their strings as str(x) shows them)."""
+    from ..shared import invalid_rules as R
+    col = fr.column(c)
+    if col.dictionary is not None:
+        codes = R.dictionary_table(col.dictionary, rule)
+        return codes, [str(col.dictionary[i]) for i in codes]
+    if rule.flags_nothing:
+        table = np.zeros(0, engine._NP_OF_ANV[col.anv_dtype])
+    elif rule.auto_only and col.anv_dtype in (_lib.ANV_I32, _lib.ANV_I64):
+        table = R.int_auto_table(engine._NP_OF_ANV[col.anv_dtype])
+    else:
+        table = R.numeric_table(_distinct_numeric(fr, c), rule)
+    is_float = col.anv_dtype in (_lib.ANV_F32, _lib.ANV_F64)
+    return table, [R.value_str(x, is_float) for x in table.tolist()]
+
+
+def _with_flags_nulled(fr, cols, bitmaps, counts, output_mode, append_cols, schema=False):
+    """The null-replacement frame: each column of `cols` (processing order) with its flagged rows nulled, the same device
+    data under a new bitmap.  replace: the column moves to the end of the frame (the reference drops it and re-adds it);
+    append: <c>_invalid is appended for the columns in `append_cols`.  schema=True: names, dtypes and dictionaries only
+    (the schema of a row-partitioned result)."""
+    new = OrderedDict((n, fr.column(n)) for n in fr.columns)
+    for c, bm, cnt in zip(cols, bitmaps, counts):
+        if output_mode == "append" and c not in append_cols:
+            continue
+        src = fr.column(c)
+        base = src.null_count if src.null_count is not None else (None if src.has_validity else 0)
+        if schema:
+            d = v = nulls = None
+        elif bm is None:                   # an empty table: the column's own validity
+            d, v = src.device()
+            nulls = base
+        else:
+            d, v = src.device()
+            nulls = None if base is None else base + int(np.sum(cnt))
+        name = c if output_mode == "replace" else c + "_invalid"
+        if output_mode == "replace":
+            del new[c]
+        new[name] = Column(name, src.sdtype, fr.n_rows, dev=d, dev_valid=bm if bm is not None else v,
+                           anv_dtype=src.anv_dtype, null_count=nulls, dictionary=src.dictionary)
+    return ColumnFrame(new, fr.n_rows)
+
+
+def invalidEntries_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_type="auto", invalid_entries=[],
+                             valid_entries=[], partial_match=False, treatment=False, treatment_method="null_replacement",
+                             treatment_configs={}, stats_missing={}, stats_unique={}, stats_mode={}, output_mode="replace",
+                             print_impact=False):
+    """reference :1342-1711, same arguments, errors and outputs.  Every verdict depends on one value only, so the host
+    decides once which distinct values are invalid (shared/invalid_rules.py: per dictionary entry for string columns,
+    a closed-form table for int / bigint columns in auto mode, the column's distinct values otherwise) and one pass on
+    the device (csrc/invalid.cu) counts the rows holding each of them and writes the nulled bitmaps of the treatment.
+
+    Orders are deterministic where the reference's are not: the rows of odf_print follow the first-seen order of
+    list_of_cols (the reference goes through a set()), and invalid_entries lists the values in table order - dictionary
+    code order for strings, ascending numeric order for numbers (Spark's distinct() order is arbitrary).  In manual /
+    both mode each value gets one verdict per column (the reference's UDF can flag one value twice and shift the flags of
+    every later column; DESIGN.md section 1).  `treatment_threshold` is popped from treatment_configs, as the reference
+    does, so the caller's dict loses it.  "all" takes the string / int / bigint / long columns; float and double columns
+    are checked when listed."""
+    from ..shared.invalid_rules import Rule
+    fr = as_frame(idf)
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        list_of_cols = [n for n, t in fr.dtypes if t in ("string", "int", "bigint", "long")]
+    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    if any(c not in fr.columns for c in cols):
+        raise TypeError("Invalid input for Column(s)")
+    if not cols:
+        warnings.warn("No Invalid Entries Check - No discrete column(s) to analyze")
+        return fr, ResultFrame(pd.DataFrame(columns=_INVALID_PRINT_COLS))
+    if output_mode not in ("replace", "append"):
+        raise TypeError("Invalid input for output_mode")
+    treatment = _as_bool(treatment, "treatment")
+    if treatment_method not in ("MMM", "null_replacement", "column_removal"):
+        raise TypeError("Invalid input for method_type")
+    threshold = treatment_configs.pop("treatment_threshold", None)
+    if threshold:
+        threshold = float(threshold)
+    elif treatment_method == "column_removal":
+        raise TypeError("Invalid input for column removal threshold")
+    bad = [c for c in cols if fr.column(c).kind == "other" or fr.column(c).sdtype.startswith("decimal")]
+    if bad:
+        raise TypeError("Column(s) %s have dtypes invalidEntries_detection does not check on the GPU path (%s); it takes "
+                        "string, integer and floating columns" % (",".join(bad), ",".join(fr.column(c).sdtype for c in bad)))
+
+    rule = Rule(detection_type, invalid_entries, valid_entries, partial_match)
+    tables, strings = zip(*[_invalid_table(fr, c, rule) for c in cols])
+    partitioned = getattr(fr, "is_partitioned", False)
+    nulling = treatment and treatment_method in ("null_replacement", "MMM")
+    counts, bitmaps = engine.flag_members(fr, cols, tables, nulling and not partitioned)
+    n = fr.count()
+    rows = []
+    for c, cnt, s in zip(cols, counts, strings):
+        hit = [s[i] for i in np.flatnonzero(cnt)]
+        total = int(cnt.sum())
+        rows.append([c, "|".join(dict.fromkeys(hit)), total, round(total / n, 4)])
+    odf_print = ResultFrame(pd.DataFrame(rows, columns=_INVALID_PRINT_COLS))
+
+    odf = fr
+    if treatment:
+        pct = {r[0]: r[3] for r in rows}
+        threshold_cols = [c for c in cols if pct[c] > threshold] if threshold else []
+        if nulling:
+            sel = [i for i, c in enumerate(cols) if not threshold or c in threshold_cols]
+            tcols = [cols[i] for i in sel]
+            append_cols = {c for c in tcols if pct[c] != 0.0}
+            if partitioned:
+                ttables = [tables[i] for i in sel]
+
+                def treat(ch):
+                    cnt, bms = engine.flag_members(ch, tcols, ttables, bool(ch.n_rows))
+                    return _with_flags_nulled(ch, tcols, bms, cnt, output_mode, append_cols)
+                odf = fr.map_chunks(_with_flags_nulled(fr._schema, tcols, [None] * len(tcols), [0] * len(tcols),
+                                                       output_mode, append_cols, schema=True), treat)
+            else:
+                odf = _with_flags_nulled(fr, tcols, [bitmaps[i] for i in sel], [counts[i] for i in sel], output_mode,
+                                         append_cols)
+        if treatment_method == "column_removal":
+            odf = fr.drop(threshold_cols)
+            if print_impact:
+                print("Removed Columns: ", threshold_cols)
+        if treatment_method == "MMM":
+            from ..data_transformer.transformers import imputation_MMM
+            from .stats_generator import uniqueCount_computation
+            if stats_unique == {} or output_mode == "append":
+                uq = uniqueCount_computation(spark, odf, cols).toPandas()
+            else:
+                uq = _read_stats(stats_unique, ["attribute", "unique_values"])
+            remove = set(uq.loc[uq["unique_values"] < 2, "attribute"].tolist())
+            cols = [c for c in cols if c not in remove]
+            if threshold:
+                cols = [c for c in threshold_cols if c not in remove]
+            if output_mode == "append" and cols:
+                cols = [c + "_invalid" for c in cols]
+            odf = imputation_MMM(spark, odf, cols, **treatment_configs, stats_missing=stats_missing, stats_mode=stats_mode,
+                                 print_impact=print_impact)
+    if print_impact:
+        odf_print.show(len(cols))
+    return odf, odf_print

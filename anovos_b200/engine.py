@@ -1088,3 +1088,71 @@ def one_hot(frame: ColumnFrame, names, indexes, ks):
           nbytes=nbytes)
     launch_count += 1
     return [o[:, :frame.n_rows] for o in outs]
+
+
+# ---- table membership (invalidEntries_detection) --------------------------------------------------
+
+_FLAG_SPEC_DT = np.dtype([("keys", "<u8"), ("n_keys", "<i8"), ("counts", "<u8"), ("out_valid", "<u8")])
+
+
+def flag_smem_keys() -> int:
+    """Largest table anv_flag_members searches in shared memory (larger ones are searched in global memory)."""
+    return int(_lib.lib().anv_flag_members_smem_keys())
+
+
+def flag_members(frame: ColumnFrame, names, tables, want_bitmap):
+    """anv_flag_members: tables = per name, a host array of the column's own dtype (int32 codes for string columns) holding
+    distinct values in ascending key order (shared/invalid_rules.sort_table).  A valid row holding a table value is a hit.
+    -> (list of uint64 ndarrays of per-entry row counts, list of int32 bitmap tensors [ceil(n_rows/32)] with the hits
+    nulled, or None where want_bitmap is False or the table is empty: an empty table is never launched and leaves the
+    column's own validity)."""
+    if getattr(frame, "is_partitioned", False):
+        if want_bitmap:
+            raise ValueError("flag_members: a row-partitioned frame counts only; map_chunks gives the treated chunks")
+        return frame.flag_members(list(names), list(tables)), [None] * len(list(names))
+    from .shared.invalid_rules import ordered_keys
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    names, tables = list(names), list(tables)
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: flag_members(frame, names[lo:hi], tables[lo:hi], want_bitmap), len(names))
+    n_words = (frame.n_rows + 31) // 32
+    keys = []
+    for n, t in zip(names, tables):
+        col = frame.column(n)
+        want = _NP_OF_ANV.get(col.anv_dtype)
+        if want is None or np.asarray(t).dtype != want:
+            raise ValueError("flag_members: column %r needs a table of %s values" % (n, want))
+        k = ordered_keys(np.asarray(t))
+        if len(k) > 1 and not bool(np.all(k[1:] > k[:-1])):
+            raise ValueError("flag_members: the table of column %r is not distinct values in key order" % n)
+        keys.append(k)
+    launch = [i for i, k in enumerate(keys) if len(k) and frame.n_rows]
+    counts = [np.zeros(len(k), np.uint64) for k in keys]
+    valid = [None] * len(names)
+    if not launch:
+        return counts, valid
+    if want_bitmap:
+        for i in launch:
+            valid[i] = torch.empty(max(n_words, 1), dtype=torch.int32, device="cuda")
+    offs = np.cumsum([0] + [len(keys[i]) for i in launch])
+    dcounts = torch.zeros(max(int(offs[-1]), 1), dtype=torch.int64, device="cuda")
+    buf, addr = _tables_to_dev([keys[i] for i in launch])
+    sp = np.zeros(len(launch), _FLAG_SPEC_DT)
+    for j, i in enumerate(launch):
+        sp[j] = (addr[j], len(keys[i]), dcounts.data_ptr() + 8 * int(offs[j]),
+                 valid[i].data_ptr() if valid[i] is not None else 0)
+    lnames = [names[i] for i in launch]
+    desc, keep = frame.descriptors(lnames)
+    nbytes = input_bytes(frame, lnames)
+    if timer is not None and want_bitmap:
+        nbytes += len(launch) * n_words * 4
+    dspecs = _to_dev(sp)                                # held until the launch is enqueued
+    _call(L.anv_flag_members, "anv_flag_members", desc.data_ptr(), dspecs.data_ptr(), len(launch), frame.n_rows, _stream(),
+          nbytes=nbytes)
+    launch_count += 1
+    flat = _host(dcounts).view(np.uint64)
+    for j, i in enumerate(launch):
+        counts[i] = flat[offs[j]:offs[j + 1]].copy()
+    return counts, [None if v is None else v[:n_words] for v in valid]

@@ -311,6 +311,21 @@ class PartitionedFrame:
             acc = [flat[offs[i]:offs[i + 1]] for i in range(len(acc))]
         return acc
 
+    def flag_members(self, names, tables):
+        """Per-entry row counts of engine.flag_members summed over the chunks and, for row slabs, over the ranks (one
+        all_reduce).  The treated chunks come from map_chunks with engine.flag_members per chunk."""
+        from . import engine
+        names, tables = list(names), list(tables)
+        acc = [np.zeros(len(t), np.uint64) for t in tables]
+        for ch in self.chunks(names):
+            counts, _ = engine.flag_members(ch, names, tables, False)
+            acc = [a + c for a, c in zip(acc, counts)]
+        if self.group is not None and names:
+            flat = self.group.all_reduce(np.concatenate(acc + [np.zeros(1, np.uint64)]))
+            offs = np.cumsum([0] + [len(a) for a in acc])
+            acc = [flat[offs[i]:offs[i + 1]].copy() for i in range(len(acc))]
+        return acc
+
     def hll_registers(self, names, p):
         from . import engine
         names = list(names)

@@ -411,6 +411,26 @@ typedef struct {
 } anv_one_hot_spec_t;
 int anv_one_hot(const anv_column_t* cols, const anv_one_hot_spec_t* specs, int n_cols, int64_t n_rows, void* stream);
 
+/* ---- table membership (invalidEntries_detection, data_analyzer/quality_checker.py:1342-1711).  Every row's value becomes
+ *      an unsigned key whose order is numeric order: ANV_I32 / ANV_I64 (dictionary codes included) flip the sign bit;
+ *      ANV_F32 / ANV_F64 first turn every NaN into the quiet NaN 0x7fc00000 / 0x7ff8000000000000, then flip all bits when
+ *      the sign is set and the sign bit otherwise (-0.0 and 0.0 are two keys, NaN sorts above +inf).
+ * anv_flag_members: keys [dev] n_keys distinct keys in ascending order, 32-bit for ANV_I32 / ANV_F32 columns and 64-bit
+ * for ANV_I64 / ANV_F64 ones, 16-byte aligned.  A valid row whose key is in the table adds 1 to counts[its index]
+ * (counts [dev] n_keys uint64, zeroed by the caller: the pass adds to them).  out_valid [dev] ceil(n_rows/32) words or
+ * NULL: with it, row r's bit is valid(r) && !hit(r) (bits past n_rows are 0).  Null rows never hit.  A spec with
+ * n_keys <= 0 or >= 2^31 or a missing keys / counts pointer leaves its column untouched.  Tables of at most
+ * anv_flag_members_smem_keys() entries are searched in shared memory, larger ones in global memory.  specs [dev] n_cols,
+ * n_cols <= ANV_MAX_LAUNCH_COLS. */
+typedef struct {
+  const void* keys;              /* [dev] n_keys ordered keys */
+  int64_t n_keys;
+  unsigned long long* counts;    /* [dev] n_keys per-entry row counts */
+  uint32_t* out_valid;           /* [dev] output bitmap, or NULL to count only */
+} anv_flag_spec_t;
+int anv_flag_members(const anv_column_t* cols, const anv_flag_spec_t* specs, int n_cols, int64_t n_rows, void* stream);
+int anv_flag_members_smem_keys(void);
+
 /* ---- Spark's Bernoulli row sampler (the DEFAULT path of drift_detector.statistics: use_sampling=True ->
  *      data_sampling.py:122-149 `idf.sample(False, fraction, seed)` / `stat.sampleBy("merge", fractions, seed)`,
  *      drift_detector.py:187-211).  One partition per call: Spark seeds XORShiftRandom with seed + partitionIndex,
