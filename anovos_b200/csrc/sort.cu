@@ -18,20 +18,17 @@
 //            the merge kernel splices the zero run back and reads the requested order statistics.
 // Counting is integer everywhere => deterministic.  Ties for the mode resolve to the
 // smallest value (the reference's choice is arbitrary, stats_generator.py:358).
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "hll_hash.cuh"
 #include "keysort.cuh"
 
 namespace anv {
 
-#ifndef ANV_SCAT_MINB
-#define ANV_SCAT_MINB 2          // resident scatter CTAs per SM the register budget is tuned for
-#endif
-// 3 compiles to 40 registers with 48 bytes of spills in sort_scatter_kernel<uint32> (12 bytes with the ranks held as 16-bit
-// halves).  It gained 0.3 % at the bench shape (H100 80GB HBM3, 400 W, sort call of 40 M x 150 float32: 72.2-72.4 ms against
-// 72.4-72.7 ms) and 1.5 % at 100 M x 12 (40.1-40.2 against 40.7-40.8 ms), so 2 stays: 64 registers, no spills.
+// Resident scatter CTAs per SM the register budget is tuned for.  3 compiles to 40 registers with 48 bytes of spills in
+// sort_scatter_kernel<uint32> (12 bytes with the ranks held as 16-bit halves).  It gained 0.3 % at the bench shape (H100 80GB
+// HBM3, 400 W, sort call of 40 M x 150 float32: 72.2-72.4 ms against 72.4-72.7 ms) and 1.5 % at 100 M x 12 (40.1-40.2
+// against 40.7-40.8 ms), so 2 stays: 64 registers, no spills.
+constexpr int SCAT_MINB = 2;
 constexpr int SORT_TILE = 4096;  // keys per CTA
 constexpr int SCAT_THREADS = 512;  // the scatter kernel runs 16 warps x 8 rounds of 32 keys
 constexpr int SCAT_WARPS = SCAT_THREADS / 32;
@@ -102,7 +99,6 @@ struct ColState {               // one per column, in the workspace
   int cur;                      // which ping-pong buffer holds the current order
   int src[8];                   // per pass: source buffer
   int skip[8];                  // per pass: digit constant -> no scatter
-  int error;                    // look-back spin limit hit (never expected): the host raises instead of hanging
 };
 
 template <typename K> struct TileSummary {
@@ -121,16 +117,11 @@ template <typename K> struct SortParams {
   uint32_t* tile_hist;          // [n_cols][256][n_tiles]  (digit-major)
   TileSummary<K>* summ;         // [n_cols][n_tiles]
   int pass;
-  // one-sweep passes (decoupled look-back): no tile-histogram and no scan kernel
-  uint32_t* ghist;              // [n_cols][sizeof(K)][256]  digit counts of the whole column, all passes, taken by pack_kernel
-  uint32_t* gbase;              // [n_cols][sizeof(K)][256]  their exclusive scans
-  unsigned long long* status;   // [n_cols][n_tiles][256]   (epoch << 56 | kind << 54 | count): tile aggregates / inclusive prefixes
-  uint32_t* ticket;             // [n_cols][sizeof(K)]       tile ids are handed out in arrival order
   // optional by-product: HyperLogLog++ registers (Spark's approx_count_distinct) from the DISTINCT sorted keys
   int hll_p;                    // 0 = off; 4..12
   uint32_t* hll_regs;           // [n_cols][1 << hll_p], zeroed by the host wrapper
 };
-constexpr int PACK_TPC = 8;     // tiles per pack CTA (amortises the flush of the digit histograms)
+constexpr int PACK_TPC = 8;     // tiles per pack CTA
 
 // byte `pass` of the key: ONE PRMT (selector nibble 0 = the byte, the other result bytes come from the zero operand)
 // instead of a shift and a mask - the digit is extracted three times per key and pass in the scatter.
@@ -144,108 +135,11 @@ template <> __device__ __forceinline__ uint32_t digit_of<uint64_t>(uint64_t k, i
 }
 
 // ---- pack: values -> keys, nulls dropped --------------------------------------------------
-// One CTA per 4096-row tile: 128-bit loads, block-level compaction (one atomicAdd per CTA
-// reserves the output range; the order before a sort is irrelevant), 64-byte runs per thread.
+// Each CTA packs PACK_TPC consecutive 4096-row tiles: block-level compaction (one atomicAdd per tile reserves the output
+// range; the order before a sort is irrelevant).
 // Exact zeros are COUNTED here instead of being sorted: sparse / zero-inflated columns (70 % zeros in the
 // benchmark's fourth family, > 90 % in the income dataset's capital-gain / capital-loss) then sort only their
 // nonzero values; run_merge_kernel splices the zero run back into mode, distinct count and ranks.
-template <typename K, typename T>
-__device__ __forceinline__ void pack_tile(const SortParams<K>& P, const anv_column_t& col, int c, const int64_t tile, uint32_t* s_warp,
-                                          unsigned long long* s_base, K* sk, uint32_t (*s_dh)[256]) {
-  constexpr int VEC = Traits<T>::VEC;
-  constexpr int PER = SORT_TILE / ANV_BLOCK;  // 16 rows per thread, contiguous
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t r0 = tile * SORT_TILE;
-  const int n_tile = (int)min((int64_t)SORT_TILE, P.n_rows - r0);
-  const T* __restrict__ data = reinterpret_cast<const T*>(col.data) + r0;
-  const uint32_t* __restrict__ vbits = col.validity;
-  const int row0 = tid * PER;
-  K keys[PER];
-  uint32_t okmask = 0;
-  if (row0 + PER <= n_tile) {
-    uint32_t vb = 0xFFFFu;
-    if (vbits) {
-      const int64_t g = r0 + row0;  // multiple of 16
-      vb = (__ldg(vbits + (g >> 5)) >> (g & 31)) & 0xFFFFu;
-    }
-    okmask = vb;
-    const uint4* p = reinterpret_cast<const uint4*>(data + row0);
-#pragma unroll
-    for (int v = 0; v < PER / VEC; ++v) {
-      const uint4 q = ldg_stream(p + v);
-      T e[VEC];
-      unpack<T>(q, e);
-#pragma unroll
-      for (int i = 0; i < VEC; ++i) keys[v * VEC + i] = make_key<K, T>(e[i]);
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < PER; ++i) {
-      const int row = row0 + i;
-      bool ok = row < n_tile;
-      keys[i] = 0;
-      if (ok) {
-        if (vbits) { const int64_t g = r0 + row; ok = (vbits[g >> 5] >> (g & 31)) & 1u; }
-        keys[i] = make_key<K, T>(data[row]);
-      }
-      okmask |= ok ? (1u << i) : 0u;
-    }
-  }
-  {  // take the zeros out (0.0 and -0.0 share one key; integers: 0)
-    constexpr K ZERO_KEY = (K)1 << (sizeof(K) * 8 - 1);
-    uint32_t zmask = 0;
-#pragma unroll
-    for (int i = 0; i < PER; ++i) zmask |= (keys[i] == ZERO_KEY) ? (1u << i) : 0u;
-    zmask &= okmask;
-    okmask &= ~zmask;
-    const uint32_t wz = __reduce_add_sync(ANV_FULL, (uint32_t)__popc(zmask));
-    if (lane == 0 && wz) atomicAdd(&P.state[c].n_zero, (unsigned long long)wz);
-  }
-  // block exclusive scan of the per-thread valid counts
-  const uint32_t mine = __popc(okmask);
-  uint32_t inc = mine;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t t = __shfl_up_sync(ANV_FULL, inc, o);
-    if (lane >= o) inc += t;
-  }
-  if (lane == 31) s_warp[warp] = inc;
-  __syncthreads();
-  if (tid == 0) {
-    uint32_t acc = 0;
-    for (int w = 0; w < ANV_WARPS; ++w) { const uint32_t t = s_warp[w]; s_warp[w] = acc; acc += t; }
-    *s_base = acc ? atomicAdd(&P.state[c].n_valid, (unsigned long long)acc) : 0ull;
-  }
-  __syncthreads();
-  // stage the compacted keys in shared memory, then write them out coalesced
-  uint32_t o = s_warp[warp] + (inc - mine);
-#pragma unroll
-  for (int i = 0; i < PER; ++i)
-    if ((okmask >> i) & 1u) sk[o++] = keys[i];
-  __shared__ uint32_t s_total;
-  if (tid == ANV_BLOCK - 1) s_total = s_warp[warp] + inc;
-  __syncthreads();
-  K* __restrict__ out = P.buf[0] + (size_t)c * P.stride + *s_base;
-  const uint32_t total = s_total;
-  // copy-out + the digit histograms of EVERY pass from the staged keys (the one-sweep passes need the column-wide digit counts
-  // before the first scatter; taking them here replaces one full read of the keys per pass)
-  if (P.ghist) {
-    for (uint32_t i = tid; i < total; i += ANV_BLOCK) {
-      const K k = sk[i];
-      out[i] = k;
-#pragma unroll
-      for (int ps = 0; ps < (int)sizeof(K); ++ps) atomicAdd(&s_dh[ps][digit_of(k, ps)], 1u);
-    }
-  } else {
-    for (uint32_t i = tid; i < total; i += ANV_BLOCK) out[i] = sk[i];
-  }
-  __syncthreads();   // sk / s_warp are reused by the CTA's next tile
-}
-
-// Strided variant (ANV_PACK_STRIDED): thread t takes rows t, t + 256, ... of the tile (coalesced scalar loads, the bitmap
-// word of a warp's 32 rows is one broadcast load), a ballot per round ranks the surviving keys of the warp, and the staging
-// stores land on CONSECUTIVE shared-memory words per warp.  The contiguous variant above (16 consecutive rows per thread)
-// writes its staging stores 16 words apart - two banks per warp, 16-way conflicts (ncu: mio_throttle is its top stall).
 template <typename T> __device__ __forceinline__ T ld_stream_scalar(const T* p);
 template <> __device__ __forceinline__ float ld_stream_scalar<float>(const float* p) {
   float v; asm volatile("ld.global.nc.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p)); return v;
@@ -260,9 +154,13 @@ template <> __device__ __forceinline__ int64_t ld_stream_scalar<int64_t>(const i
   long long v; asm volatile("ld.global.nc.L1::no_allocate.s64 %0, [%1];" : "=l"(v) : "l"(p)); return (int64_t)v;
 }
 
+// Thread t takes rows t, t + 256, ... of the tile (coalesced scalar loads, the bitmap word of a warp's 32 rows is one
+// broadcast load), a ballot per round ranks the surviving keys of the warp, and the staging stores land on CONSECUTIVE
+// shared-memory words per warp: no bank conflicts.  16 consecutive rows per thread would put a warp's staging stores 16
+// words apart, 16-way conflicts (100 M x 12 float32, whole sort call: 27.29 ms against 26.38 ms for this layout, B200).
 template <typename K, typename T>
-__device__ __forceinline__ void pack_tile_strided(const SortParams<K>& P, const anv_column_t& col, int c, const int64_t tile, uint32_t* s_warp,
-                                                  unsigned long long* s_base, K* sk, uint32_t (*s_dh)[256]) {
+__device__ __forceinline__ void pack_tile(const SortParams<K>& P, const anv_column_t& col, int c, const int64_t tile, uint32_t* s_warp,
+                                          unsigned long long* s_base, K* sk) {
   constexpr int PER = SORT_TILE / ANV_BLOCK;        // 16 rounds of 256 rows
   constexpr int WREG = SORT_TILE / ANV_WARPS;       // a warp stages at most 16 x 32 keys: its own 512 slots of sk
   constexpr K ZERO_KEY = (K)1 << (sizeof(K) * 8 - 1);
@@ -288,7 +186,7 @@ __device__ __forceinline__ void pack_tile_strided(const SortParams<K>& P, const 
   for (int i = 0; i < PER; ++i) {
     const K k = make_key<K, T>(x[i]);
     bool ok = (__shfl_sync(ANV_FULL, wv, i) & lbit) != 0u;
-    if (!full) ok = ok && (i * ANV_BLOCK + tid) < n_tile;
+    ok = ok && (full || (i * ANV_BLOCK + tid) < n_tile);   // a select: as a branch, nvcc duplicates the 16 rounds for full tiles
     const bool zero = ok && k == ZERO_KEY;          // 0.0 and -0.0 share one key; integers: 0
     nzero += zero ? 1u : 0u;
     ok = ok && !zero;
@@ -308,117 +206,41 @@ __device__ __forceinline__ void pack_tile_strided(const SortParams<K>& P, const 
   __syncthreads();
   // every warp copies its own staged keys out (the order before a sort is irrelevant): contiguous, coalesced
   K* __restrict__ out = P.buf[0] + (size_t)c * P.stride + *s_base + s_warp[warp];
-  if (P.ghist) {
-    for (uint32_t j = lane; j < wcount; j += 32) {
-      const K k = mine[j];
-      out[j] = k;
-#pragma unroll
-      for (int ps = 0; ps < (int)sizeof(K); ++ps) atomicAdd(&s_dh[ps][digit_of(k, ps)], 1u);
-    }
-  } else {
-    for (uint32_t j = lane; j < wcount; j += 32) out[j] = mine[j];
-  }
+  for (uint32_t j = lane; j < wcount; j += 32) out[j] = mine[j];
   __syncthreads();   // sk / s_warp / s_base are reused by the CTA's next tile
 }
 
-#ifndef ANV_PACK_STRIDED
-#define ANV_PACK_STRIDED 1   // measured (100 M x 12 float32, whole sort call): contiguous 27.29 ms, strided 26.38 ms, identical results
-#endif
-#if ANV_PACK_STRIDED
-#define ANV_PACK_TILE pack_tile_strided
-#else
-#define ANV_PACK_TILE pack_tile
-#endif
-
-#ifndef ANV_PACK_MINB
-#define ANV_PACK_MINB 6        // 40 registers, no spills for 32-bit keys (1: 26.64 ms, 5: 26.44, 6: 26.38); 64-bit keys: 5
-#endif
+// Resident pack CTAs per SM: 32-bit keys compile to 40 registers, no spills at 6 (B200, 100 M x 12 float32, whole sort call:
+// 1: 26.64 ms, 5: 26.44, 6: 26.38); 64-bit keys: 5.
+template <typename K> constexpr int PACK_MINB = sizeof(K) == 8 ? 5 : 6;
 template <typename K>
-__global__ void __launch_bounds__(ANV_BLOCK, (sizeof(K) == 8 && ANV_PACK_MINB > 5) ? 5 : ANV_PACK_MINB) pack_kernel(const SortParams<K> P) {
+__global__ void __launch_bounds__(ANV_BLOCK, PACK_MINB<K>) pack_kernel(const SortParams<K> P) {
   __shared__ uint32_t s_warp[ANV_WARPS];
   __shared__ unsigned long long s_base;
   __shared__ K sk[SORT_TILE];
-  __shared__ uint32_t s_dh[sizeof(K)][256];
-  const int c = blockIdx.y, tid = threadIdx.x;
+  const int c = blockIdx.y;
   const anv_column_t col = P.cols[c];
-#pragma unroll
-  for (int ps = 0; ps < (int)sizeof(K); ++ps) s_dh[ps][tid] = 0;
-  __syncthreads();
   for (int t = 0; t < PACK_TPC; ++t) {
     const int64_t tile = (int64_t)blockIdx.x * PACK_TPC + t;
     if (tile * SORT_TILE >= P.n_rows) break;
     switch (col.dtype) {
-      case ANV_F32: ANV_PACK_TILE<K, float>(P, col, c, tile, s_warp, &s_base, sk, s_dh); break;
-      case ANV_I32: ANV_PACK_TILE<K, int32_t>(P, col, c, tile, s_warp, &s_base, sk, s_dh); break;
-      case ANV_F64: if (sizeof(K) == 8) ANV_PACK_TILE<K, double>(P, col, c, tile, s_warp, &s_base, sk, s_dh); break;
-      case ANV_I64: if (sizeof(K) == 8) ANV_PACK_TILE<K, int64_t>(P, col, c, tile, s_warp, &s_base, sk, s_dh); break;
+      case ANV_F32: pack_tile<K, float>(P, col, c, tile, s_warp, &s_base, sk); break;
+      case ANV_I32: pack_tile<K, int32_t>(P, col, c, tile, s_warp, &s_base, sk); break;
+      case ANV_F64: if (sizeof(K) == 8) pack_tile<K, double>(P, col, c, tile, s_warp, &s_base, sk); break;
+      case ANV_I64: if (sizeof(K) == 8) pack_tile<K, int64_t>(P, col, c, tile, s_warp, &s_base, sk); break;
       default: break;
     }
-  }
-  if (!P.ghist) return;
-  __syncthreads();
-  uint32_t* g = P.ghist + (size_t)c * sizeof(K) * 256;
-#pragma unroll
-  for (int ps = 0; ps < (int)sizeof(K); ++ps) {
-    const uint32_t v = s_dh[ps][tid];
-    if (v) atomicAdd(&g[ps * 256 + tid], v);
-  }
-}
-
-// Column-wide exclusive digit offsets of every pass + which passes are no-ops (one digit holds every key) + the ping-pong
-// buffer each pass reads: everything the one-sweep passes need is known after the pack kernel.
-template <typename K>
-__global__ void __launch_bounds__(ANV_BLOCK) sort_bases_kernel(const SortParams<K> P) {
-  const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  ColState& S = P.state[c];
-  const unsigned long long n = S.n_valid;
-  __shared__ uint32_t wsum[ANV_WARPS];
-  __shared__ int s_skip[sizeof(K)];
-  if (tid < (int)sizeof(K)) s_skip[tid] = (n == 0) ? 1 : 0;
-  __syncthreads();
-  for (int ps = 0; ps < (int)sizeof(K); ++ps) {
-    const uint32_t v = P.ghist[((size_t)c * sizeof(K) + ps) * 256 + tid];
-    if (n > 0 && (unsigned long long)v == n) s_skip[ps] = 1;
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(ANV_FULL, inc, o); if (lane >= o) inc += t; }
-    if (lane == 31) wsum[warp] = inc;
-    __syncthreads();
-    uint32_t woff = 0;
-#pragma unroll
-    for (int w = 0; w < ANV_WARPS; ++w) woff += (w < warp) ? wsum[w] : 0u;
-    P.gbase[((size_t)c * sizeof(K) + ps) * 256 + tid] = woff + inc - v;
-    __syncthreads();
-  }
-  if (tid == 0) {
-    int cur = 0;
-    for (int ps = 0; ps < (int)sizeof(K); ++ps) {
-      S.src[ps] = cur;
-      S.skip[ps] = s_skip[ps];
-      if (!s_skip[ps]) cur ^= 1;
-    }
-    S.cur = cur;
   }
 }
 
 // Lanes of `act` holding the same 8-bit digit.
-// Default: per bit, one small NON-volatile asm block (and, setp, vote.ballot.sync, @!p not) gives the lanes whose bit equals
+// Per bit, one small NON-volatile asm block (and, setp, vote.ballot.sync, @!p not) gives the lanes whose bit equals
 // mine, and the 8 masks are ANDed in C++.  ptxas turns this into R2P (7 digit bits into predicates at once), VOTE, a
 // predicated NOT and a LOP3 AND: about 3 instructions per bit.  The same ballots written with __ballot_sync and a C++
 // select compile to 6-7 per bit.  ptxas 12.9 for sm_90a does not finish the scatter kernels when all 8 bits sit in one asm
 // block (selp + lop3 0x60), volatile or not, nor when the ANDs are written as asm lop3 next to these blocks.
-// ANV_PEERS_MATCH=1: one MATCH.ANY over the whole warp, masked with `act` afterwards (lanes past the end of a partial tile
-// hold digit 0: they must take part in the call but match no live lane).  Fewer instructions (sort_scatter_kernel<uint32>
-// 1243 SASS against 1650) but slower on an H100 80GB HBM3 at 400 W, whole anv_mode_distinct call with ranks and HLL++,
-// two alternating runs each: 100 M x 12 float32 47.8-48.2 ms against 40.7-40.8 ms with the ballots, 40 M x 150
-// 83.2-84.5 ms against 72.4-72.7 ms (the C++ ballots before: 43.5-43.7 and 78.1-78.2 ms).
-#ifndef ANV_PEERS_MATCH
-#define ANV_PEERS_MATCH 0
-#endif
+// One __match_any_sync is fewer instructions but measured 16-18 % slower per sort call on an H100.
 __device__ __forceinline__ uint32_t peers8(uint32_t d, uint32_t act) {
-#if ANV_PEERS_MATCH
-  return __match_any_sync(ANV_FULL, d) & act;
-#else
   uint32_t m = act;
 #pragma unroll
   for (int b = 0; b < 8; ++b) {
@@ -432,19 +254,14 @@ __device__ __forceinline__ uint32_t peers8(uint32_t d, uint32_t act) {
     m &= same;
   }
   return m;
-#endif
 }
-
 
 // ---- pass step 1: per-tile digit histogram ------------------------------------------------------
 // Plain shared-memory atomics (the hardware resolves same-address lanes itself; a match_any
 // pre-aggregation only adds instructions).
-#ifndef ANV_HIST_TPC
-#define ANV_HIST_TPC 4
-#endif
-// tiles per tile-histogram CTA: the two dependent loads that start a CTA (column state, then keys) are paid once per 64 KB.
-// The same knob on the scatter and the run summaries stays at 1.
-constexpr int HIST_TPC = ANV_HIST_TPC;
+// Tiles per tile-histogram CTA: the two dependent loads that start a CTA (column state, then keys) are paid once per 64 KB.
+// The scatter and the run summaries take one tile per CTA.
+constexpr int HIST_TPC = 4;
 template <typename K>
 __global__ void __launch_bounds__(ANV_BLOCK) sort_hist_kernel(const SortParams<K> P) {
   const int c = blockIdx.y, tid = threadIdx.x;
@@ -583,34 +400,11 @@ template <typename K> struct ScatShared {   // declared ONCE in the kernel (stat
   K sk[SORT_TILE + 1];                        // + the spare slot of the branch-free placement
 };
 
-constexpr unsigned long long LB_AGG = 1ull << 54, LB_PREFIX = 2ull << 54, LB_VALUE = (1ull << 54) - 1ull;
-constexpr int LB_SPIN_LIMIT = 1 << 20;
-
-// Decoupled look-back of ONE digit: add up the aggregates of the preceding tiles until one that already knows its inclusive
-// prefix, then publish this tile's inclusive prefix.  (Not inlined: keeps the spin loop out of the scatter's control flow.)
-__device__ __noinline__ unsigned long long lookback_exclusive(volatile unsigned long long* status, int tile, int d, unsigned long long epoch,
-                                                             unsigned long long total, int* error) {
-  unsigned long long excl = 0;
-  for (int t = tile - 1; t >= 0; --t) {
-    unsigned long long v = status[(size_t)t * 256 + d];
-    int spins = 0;
-    while ((v >> 56) != (epoch >> 56)) {
-      // never expected (tiles start in ticket order); once one look-back has given up every other one follows at once
-      if (++spins > LB_SPIN_LIMIT || ((spins & 255) == 0 && *reinterpret_cast<volatile int*>(error))) { *error = 1; return excl; }
-      v = status[(size_t)t * 256 + d];
-    }
-    excl += v & LB_VALUE;
-    if (v & LB_PREFIX) break;
-  }
-  status[(size_t)tile * 256 + d] = epoch | LB_PREFIX | (excl + total);
-  return excl;
-}
-
 // store through the global window (the opaque base pointer below would otherwise compile to a generic ST)
 __device__ __forceinline__ void st_global_key(uint32_t* p, uint32_t v) { asm volatile("st.global.b32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ void st_global_key(uint64_t* p, uint64_t v) { asm volatile("st.global.b64 [%0], %1;" ::"l"(p), "l"(v) : "memory"); }
 
-template <typename K, bool FULL, bool LOOKBACK>
+template <typename K, bool FULL>
 __device__ __forceinline__ void scatter_tile(const SortParams<K>& P, const ColState& S, const int c, const int tile, const int64_t t0,
                                              const int nt_in, ScatShared<K>& SH) {
   auto& wcnt = SH.wcnt;
@@ -626,7 +420,7 @@ __device__ __forceinline__ void scatter_tile(const SortParams<K>& P, const ColSt
 #pragma unroll
   for (int j = 0; j < SCAT_WARPS * 256 / 2 / SCAT_THREADS; ++j)   // fixed trip count: 4 stores, no loop control
     reinterpret_cast<uint32_t*>(&wcnt[0][0])[tid + j * SCAT_THREADS] = 0;
-  if (!LOOKBACK && tid < 256) gbase[tid] = P.tile_hist[((size_t)c * 256 + tid) * P.n_tiles + tile];
+  if (tid < 256) gbase[tid] = P.tile_hist[((size_t)c * 256 + tid) * P.n_tiles + tile];
   constexpr int WR = SORT_TILE / SCAT_WARPS / 32;  // 8 rounds per warp
   K key[WR];
   uint32_t peers[WR];
@@ -667,11 +461,6 @@ __device__ __forceinline__ void scatter_tile(const SortParams<K>& P, const ColSt
     for (int w = 0; w < SCAT_WARPS; ++w) { const uint32_t t = wcnt[w][tid]; wcnt[w][tid] = (uint16_t)acc; acc += t; }
     total = acc;
   }
-  const unsigned long long epoch = (unsigned long long)(P.pass + 1) << 56;
-  volatile unsigned long long* const status = LOOKBACK ? P.status + ((size_t)c * P.n_tiles) * 256 : nullptr;
-  if (LOOKBACK && tid < 256)   // publish this tile's digit counts at once: its successors only need these to move on
-    status[(size_t)tile * 256 + tid] = epoch | (tile == 0 ? LB_PREFIX : LB_AGG) | (unsigned long long)total;
-  uint32_t ds_keep = 0;
   {  // exclusive scan of the 256 digit totals -> start of each digit inside the reordered tile
     uint32_t inc = total;
 #pragma unroll
@@ -690,8 +479,7 @@ __device__ __forceinline__ void scatter_tile(const SortParams<K>& P, const ColSt
       // "global base minus tile start" table for the copy-out (one lookup per key there as well)
 #pragma unroll
       for (int w = 0; w < SCAT_WARPS; ++w) wcnt[w][tid] = (uint16_t)(wcnt[w][tid] + ds);
-      if (LOOKBACK) ds_keep = ds;
-      else gbase[tid] -= ds;
+      gbase[tid] -= ds;
     }
   }
   __syncthreads();
@@ -700,10 +488,6 @@ __device__ __forceinline__ void scatter_tile(const SortParams<K>& P, const ColSt
     const uint32_t d = digit_of(key[r], P.pass);
     const uint32_t at = wcnt[warp][d] + pos[r];
     sk[(FULL || peers[r]) ? at : (uint32_t)SORT_TILE] = key[r];
-  }
-  if (LOOKBACK && tid < 256) {
-    const unsigned long long excl = lookback_exclusive(status, tile, tid, epoch, (unsigned long long)total, &P.state[c].error);
-    gbase[tid] = P.gbase[((size_t)c * sizeof(K) + P.pass) * 256 + tid] + (uint32_t)excl - ds_keep;
   }
   __syncthreads();
   // the column's output base as ONE 64-bit register pair (opaque to the compiler: it otherwise re-derives
@@ -725,48 +509,18 @@ __device__ __forceinline__ void scatter_tile(const SortParams<K>& P, const ColSt
   }
 }
 
-#ifndef ANV_SCAT_TPC
-#define ANV_SCAT_TPC 1
-#endif
-constexpr int SCAT_TPC = ANV_SCAT_TPC;   // tiles per scatter CTA (tuning knob)
 template <typename K>
-__global__ void __launch_bounds__(SCAT_THREADS, ANV_SCAT_MINB) sort_scatter_kernel(const SortParams<K> P) {
-  const int c = blockIdx.y;
+__global__ void __launch_bounds__(SCAT_THREADS, SCAT_MINB) sort_scatter_kernel(const SortParams<K> P) {
+  const int c = blockIdx.y, tile = blockIdx.x;
   const ColState& S = P.state[c];
   if (S.skip[P.pass]) return;
-  const int64_t n = (int64_t)S.n_valid;
-  __shared__ ScatShared<K> SH;
-  for (int tt = 0; tt < SCAT_TPC; ++tt) {
-    const int tile = blockIdx.x * SCAT_TPC + tt;
-    const int64_t t0 = (int64_t)tile * SORT_TILE;
-    if (t0 >= n) return;
-    const int nt = (int)min((int64_t)SORT_TILE, n - t0);
-    if (nt == SORT_TILE) scatter_tile<K, true, false>(P, S, c, tile, t0, nt, SH);
-    else scatter_tile<K, false, false>(P, S, c, tile, t0, nt, SH);
-    __syncthreads();            // the staging area and the digit tables are reused by the next tile
-  }
-}
-
-// One-sweep pass: the same stable scatter, but the tile's global digit offsets come from the column-wide digit bases
-// (sort_bases_kernel) + a decoupled look-back over the preceding tiles' digit counts - one read and one write of the keys per
-// pass, no tile-histogram kernel, no scan kernel.  Tile ids are tickets (arrival order), so every tile a CTA waits for has
-// already started: the look-back cannot deadlock.
-template <typename K>
-__global__ void __launch_bounds__(SCAT_THREADS, 2) sort_onesweep_kernel(const SortParams<K> P) {
-  const int c = blockIdx.y;
-  const ColState& S = P.state[c];
-  if (S.skip[P.pass]) return;
-  __shared__ int s_tile;
-  if (threadIdx.x == 0) s_tile = (int)atomicAdd(&P.ticket[(size_t)c * sizeof(K) + P.pass], 1u);
-  __syncthreads();
-  const int tile = s_tile;
   const int64_t n = (int64_t)S.n_valid;
   const int64_t t0 = (int64_t)tile * SORT_TILE;
   if (t0 >= n) return;
   const int nt = (int)min((int64_t)SORT_TILE, n - t0);
   __shared__ ScatShared<K> SH;
-  if (nt == SORT_TILE) scatter_tile<K, true, true>(P, S, c, tile, t0, nt, SH);
-  else scatter_tile<K, false, true>(P, S, c, tile, t0, nt, SH);
+  if (nt == SORT_TILE) scatter_tile<K, true>(P, S, c, tile, t0, nt, SH);
+  else scatter_tile<K, false>(P, S, c, tile, t0, nt, SH);
 }
 
 // Associative combine of two ADJACENT run summaries (left, right) of sorted keys.
@@ -814,13 +568,9 @@ template <typename K> __device__ __forceinline__ TileSummary<K> shfl_down_summar
 // Each thread summarises 16 CONSECUTIVE sorted keys in registers (blocked 128-bit loads), the 256
 // thread summaries are folded with the associative `combine` (shuffle tree per warp, then 8 warps
 // sequentially): no shared-memory tile, no binary search, ~25 instructions per key.
-#ifndef ANV_RUN_TPC
-#define ANV_RUN_TPC 1
-#endif
-constexpr int RUN_TPC = ANV_RUN_TPC;     // tiles per run-summary CTA (tuning knob)
 template <typename K>
-__device__ __forceinline__ void run_tile_one(const SortParams<K>& P, const int c, const int tile) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+__global__ void __launch_bounds__(ANV_BLOCK) run_tile_kernel(const SortParams<K> P) {
+  const int c = blockIdx.y, tile = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const ColState& S = P.state[c];
   const int64_t n = (int64_t)S.n_valid;
   const int64_t t0 = (int64_t)tile * SORT_TILE;
@@ -921,16 +671,6 @@ __device__ __forceinline__ void run_tile_one(const SortParams<K>& P, const int c
   }
 }
 
-template <typename K>
-__global__ void __launch_bounds__(ANV_BLOCK) run_tile_kernel(const SortParams<K> P) {
-  for (int tt = 0; tt < RUN_TPC; ++tt) {
-    const int tile = blockIdx.x * RUN_TPC + tt;
-    if (tile >= P.n_tiles) return;
-    run_tile_one<K>(P, blockIdx.y, tile);
-    __syncthreads();           // the shared staging (head keys, warp summaries) is reused by the next tile
-  }
-}
-
 // One warp per column: 32 tile summaries per step are combined with an order-preserving
 // shuffle tree, the chunk results sequentially by lane 0.  Also reads the requested order
 // statistics straight out of the sorted keys.
@@ -971,10 +711,6 @@ __global__ void __launch_bounds__(32 * MERGE_WARPS) run_merge_kernel(const SortP
     uint32_t idx, rho;
     hll_slot(spark_hash_of_key<K>(ZERO_KEY, dt), P.hll_p, idx, rho);
     atomicMax(&P.hll_regs[((size_t)c << P.hll_p) + idx], rho);
-  }
-  if (S.error) {                      // a look-back gave up: make the host raise (results would be garbage)
-    if (tid == 0) { mode_value[c] = nan(""); mode_rows[c] = -3; n_distinct[c] = -3; }
-    return;
   }
   if (n == 0) {
     if (tid == 0) {
@@ -1023,24 +759,54 @@ __global__ void __launch_bounds__(32 * MERGE_WARPS) run_merge_kernel(const SortP
   }
 }
 
+// ---- host side ------------------------------------------------------------------------------------------------------
+// Offsets of a [n_cols][256][n_tiles] count table: the 256 totals of each column, then every entry's exclusive offset in
+// digit-major order (sort_scan_kernel also takes pass P.pass's skip decision).
+template <typename K> static void scan_tile_counts(const SortParams<K>& P, uint32_t* totals, cudaStream_t st) {
+  sort_totals_kernel<K><<<dim3(256, P.n_cols), ANV_BLOCK, 0, st>>>(P, totals);
+  sort_scan_kernel<K><<<dim3(256, P.n_cols), ANV_BLOCK, 0, st>>>(P, totals);
+}
+
+// LSD passes first_pass .. end_pass - 1 over the keys in P.buf: tile histogram, totals + scan, stable scatter.
+template <typename K> static int lsd_passes(SortParams<K>& P, uint32_t* totals, int first_pass, int end_pass, cudaStream_t st) {
+  for (int pass = first_pass; pass < end_pass; ++pass) {
+    P.pass = pass;
+    sort_hist_kernel<K><<<dim3((P.n_tiles + HIST_TPC - 1) / HIST_TPC, P.n_cols), ANV_BLOCK, 0, st>>>(P);
+    scan_tile_counts(P, totals, st);
+    sort_scatter_kernel<K><<<dim3(P.n_tiles, P.n_cols), SCAT_THREADS, 0, st>>>(P);
+    ANV_CUDA(cudaGetLastError());
+  }
+  return ANV_OK;
+}
+
 template <typename K> struct Layout {
-  size_t state, buf0, buf1, tile_hist, summ, totals, ghist, gbase, ticket, status, total;
-  Layout(int n_cols, int64_t n_rows) {
-    const int64_t stride = (n_rows + 63) & ~(int64_t)63;
-    const int64_t n_tiles = (n_rows + SORT_TILE - 1) / SORT_TILE;
+  int n_cols, n_tiles;
+  int64_t n_rows, stride;
+  size_t state, buf0, buf1, tile_hist, summ, totals, total;
+  Layout(int n_cols_, int64_t n_rows_) : n_cols(n_cols_), n_rows(n_rows_) {
+    stride = (n_rows + 63) & ~(int64_t)63;
+    const int64_t nt = (n_rows + SORT_TILE - 1) / SORT_TILE;
+    n_tiles = nt > 0 ? (int)nt : 1;
     size_t o = 0;
     auto take = [&](size_t bytes) { size_t at = o; o = (o + bytes + 255) & ~(size_t)255; return at; };
     state = take((size_t)n_cols * sizeof(ColState));
     buf0 = take((size_t)n_cols * stride * sizeof(K));
     buf1 = take((size_t)n_cols * stride * sizeof(K));
-    tile_hist = take((size_t)n_cols * 256 * (n_tiles > 0 ? n_tiles : 1) * 4);
-    summ = take((size_t)n_cols * (n_tiles > 0 ? n_tiles : 1) * sizeof(TileSummary<K>));
+    tile_hist = take((size_t)n_cols * 256 * n_tiles * 4);
+    summ = take((size_t)n_cols * n_tiles * sizeof(TileSummary<K>));
     totals = take((size_t)n_cols * 256 * 4);
-    ghist = take((size_t)n_cols * sizeof(K) * 256 * 4);     // ghist, gbase, ticket, status are contiguous: one memset
-    gbase = take((size_t)n_cols * sizeof(K) * 256 * 4);
-    ticket = take((size_t)n_cols * sizeof(K) * 4);
-    status = take((size_t)n_cols * (n_tiles > 0 ? n_tiles : 1) * 256 * 8);
     total = o + 256;
+  }
+  // the sort's parameters over workspace `w`; pass and HLL++ are the caller's
+  SortParams<K> bind(char* w, const anv_column_t* cols) const {
+    SortParams<K> P{};
+    P.cols = cols; P.n_cols = n_cols; P.n_rows = n_rows; P.stride = stride; P.n_tiles = n_tiles;
+    P.buf[0] = reinterpret_cast<K*>(w + buf0);
+    P.buf[1] = reinterpret_cast<K*>(w + buf1);
+    P.state = reinterpret_cast<ColState*>(w + state);
+    P.tile_hist = reinterpret_cast<uint32_t*>(w + tile_hist);
+    P.summ = reinterpret_cast<TileSummary<K>*>(w + summ);
+    return P;
   }
 };
 
@@ -1048,65 +814,21 @@ template <typename K>
 static int run_mode_distinct(const anv_column_t* cols, int n_cols, int64_t n_rows, double* mode_value, int64_t* mode_rows,
                              int64_t* n_distinct, const int64_t* ranks, int n_ranks, double* rank_values, int hll_p,
                              uint32_t* hll_regs, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  Layout<K> L(n_cols, n_rows);
+  const Layout<K> L(n_cols, n_rows);
   if (workspace_bytes < L.total) { set_error("anv_mode_distinct: workspace too small (%zu < %zu)", workspace_bytes, L.total); return ANV_ERR_WORKSPACE; }
   char* w = reinterpret_cast<char*>(workspace);
-  SortParams<K> P{};
-  P.cols = cols; P.n_cols = n_cols; P.n_rows = n_rows;
-  P.stride = (n_rows + 63) & ~(int64_t)63;
-  P.n_tiles = (int)((n_rows + SORT_TILE - 1) / SORT_TILE);
-  if (P.n_tiles < 1) P.n_tiles = 1;
-  P.buf[0] = reinterpret_cast<K*>(w + L.buf0);
-  P.buf[1] = reinterpret_cast<K*>(w + L.buf1);
-  P.state = reinterpret_cast<ColState*>(w + L.state);
-  P.tile_hist = reinterpret_cast<uint32_t*>(w + L.tile_hist);
-  P.summ = reinterpret_cast<TileSummary<K>*>(w + L.summ);
+  SortParams<K> P = L.bind(w, cols);
   uint32_t* totals = reinterpret_cast<uint32_t*>(w + L.totals);
-  P.ghist = nullptr;                                   // set below when the one-sweep passes are selected
-  P.gbase = reinterpret_cast<uint32_t*>(w + L.gbase);
-  P.ticket = reinterpret_cast<uint32_t*>(w + L.ticket);
-  P.status = reinterpret_cast<unsigned long long*>(w + L.status);
   P.hll_p = hll_regs ? hll_p : 0;
   P.hll_regs = hll_regs;
   if (hll_regs) ANV_CUDA(cudaMemsetAsync(hll_regs, 0, ((size_t)n_cols << hll_p) * sizeof(uint32_t), st));
-  // Default: three kernels per pass (tile histogram, (digit, column)-parallel scan, stable scatter).  ANV_SORT_ONESWEEP=1 selects the
-  // one-sweep passes for 32-bit keys (digit histograms in pack + decoupled look-back in the scatter: 10 instead of 14 words of
-  // traffic per key).  The look-back walks several predecessor tiles per digit with dependent L2 round trips while the
-  // scatter is issue-bound, not HBM-bound, so removing a read of the keys need not pay.  Kept, tested, not the default.
-  const char* os_env = getenv("ANV_SORT_ONESWEEP");
-  const bool legacy = !(os_env && os_env[0] == '1') || sizeof(K) != 4;
   ANV_CUDA(cudaMemsetAsync(P.state, 0, (size_t)n_cols * sizeof(ColState), st));
-  if (!legacy) {
-    P.ghist = reinterpret_cast<uint32_t*>(w + L.ghist);
-    ANV_CUDA(cudaMemsetAsync(w + L.ghist, 0, L.total - 256 - L.ghist, st));   // digit counts, bases, tickets, look-back status
-  }
   if (n_rows > 0) {
-    dim3 grid(P.n_tiles, n_cols);
     pack_kernel<K><<<dim3((P.n_tiles + PACK_TPC - 1) / PACK_TPC, n_cols), ANV_BLOCK, 0, st>>>(P);
     ANV_CUDA(cudaGetLastError());
-    // 64-bit keys keep the three-kernel passes: ptxas (12.9) does not terminate on the uint64 instantiation of the one-sweep kernel
-    if constexpr (sizeof(K) == 4) {
-      if (!legacy) {
-        sort_bases_kernel<K><<<n_cols, ANV_BLOCK, 0, st>>>(P);
-        for (int pass = 0; pass < (int)sizeof(K); ++pass) {
-          P.pass = pass;
-          sort_onesweep_kernel<K><<<grid, SCAT_THREADS, 0, st>>>(P);
-          ANV_CUDA(cudaGetLastError());
-        }
-      }
-    }
-    if (legacy || sizeof(K) != 4) {
-      for (int pass = 0; pass < (int)sizeof(K); ++pass) {
-        P.pass = pass;
-        sort_hist_kernel<K><<<dim3((P.n_tiles + HIST_TPC - 1) / HIST_TPC, n_cols), ANV_BLOCK, 0, st>>>(P);
-        sort_totals_kernel<K><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(P, totals);
-        sort_scan_kernel<K><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(P, totals);
-        sort_scatter_kernel<K><<<dim3((P.n_tiles + SCAT_TPC - 1) / SCAT_TPC, n_cols), SCAT_THREADS, 0, st>>>(P);
-        ANV_CUDA(cudaGetLastError());
-      }
-    }
+    if (int e = lsd_passes(P, totals, 0, (int)sizeof(K), st)) return e;
     const size_t run_smem = P.hll_p ? (size_t)SORT_TILE * sizeof(K) : 0;   // the compacted head keys
-    run_tile_kernel<K><<<dim3((P.n_tiles + RUN_TPC - 1) / RUN_TPC, n_cols), ANV_BLOCK, run_smem, st>>>(P);
+    run_tile_kernel<K><<<dim3(P.n_tiles, n_cols), ANV_BLOCK, run_smem, st>>>(P);
     ANV_CUDA(cudaGetLastError());
   }
   run_merge_kernel<K><<<n_cols, 32 * MERGE_WARPS, 0, st>>>(P, mode_value, mode_rows, n_distinct, ranks, n_ranks, rank_values);
@@ -1167,15 +889,7 @@ int key_sort64(void* workspace, size_t workspace_bytes, int64_t n_rows, int firs
   key_sort_init_kernel<<<1, 1, 0, st>>>(P.state, n_rows);
   ANV_CUDA(cudaGetLastError());
   if (n_rows == 0) return ANV_OK;
-  for (int pass = first_pass; pass < end_pass; ++pass) {
-    P.pass = pass;
-    sort_hist_kernel<uint64_t><<<dim3((P.n_tiles + HIST_TPC - 1) / HIST_TPC, 1), ANV_BLOCK, 0, st>>>(P);
-    sort_totals_kernel<uint64_t><<<dim3(256, 1), ANV_BLOCK, 0, st>>>(P, totals);
-    sort_scan_kernel<uint64_t><<<dim3(256, 1), ANV_BLOCK, 0, st>>>(P, totals);
-    sort_scatter_kernel<uint64_t><<<dim3((P.n_tiles + SCAT_TPC - 1) / SCAT_TPC, 1), SCAT_THREADS, 0, st>>>(P);
-    ANV_CUDA(cudaGetLastError());
-  }
-  return ANV_OK;
+  return lsd_passes(P, totals, first_pass, end_pass, st);
 }
 
 
@@ -2128,19 +1842,9 @@ static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_r
   if (workspace_bytes < L.total) { set_error("anv_mode_distinct_partition: workspace too small (%zu < %zu)", workspace_bytes, L.total); return ANV_ERR_WORKSPACE; }
   char* w = reinterpret_cast<char*>(workspace);
   // --- the sample sort reuses the LSD machinery on m keys per column ---
-  Layout<uint32_t> LS(n_cols, L.m);
-  char* ws = w + L.lsd;
-  SortParams<uint32_t> S{};
-  S.cols = cols; S.n_cols = n_cols; S.n_rows = L.m;
-  S.stride = (L.m + 63) & ~(int64_t)63;
-  S.n_tiles = (int)((L.m + SORT_TILE - 1) / SORT_TILE);
-  if (S.n_tiles < 1) S.n_tiles = 1;
-  S.buf[0] = reinterpret_cast<uint32_t*>(ws + LS.buf0);
-  S.buf[1] = reinterpret_cast<uint32_t*>(ws + LS.buf1);
-  S.state = reinterpret_cast<ColState*>(ws + LS.state);
-  S.tile_hist = reinterpret_cast<uint32_t*>(ws + LS.tile_hist);
-  S.summ = reinterpret_cast<TileSummary<uint32_t>*>(ws + LS.summ);
-  uint32_t* sample_totals = reinterpret_cast<uint32_t*>(ws + LS.totals);
+  const Layout<uint32_t> LS(n_cols, L.m);
+  SortParams<uint32_t> S = LS.bind(w + L.lsd, cols);
+  uint32_t* sample_totals = reinterpret_cast<uint32_t*>(w + L.lsd + LS.totals);
   PcParams P{};
   P.cols = cols; P.n_cols = n_cols; P.n_rows = n_rows; P.stride = L.stride; P.n_tiles = L.n_tiles;
   P.P = L.P; P.NS = L.NS; P.NB = L.NB; P.G = L.G; P.max_chunks = L.max_chunks; P.m = L.m;
@@ -2173,21 +1877,13 @@ static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_r
     dim3 grid((unsigned)((L.m + ANV_BLOCK - 1) / ANV_BLOCK), n_cols);
     pc_sample_kernel<<<grid, ANV_BLOCK, 0, st>>>(S, n_rows, L.m);
     ANV_CUDA(cudaGetLastError());
-    for (int pass = 0; pass < 4; ++pass) {
-      S.pass = pass;
-      sort_hist_kernel<uint32_t><<<dim3((S.n_tiles + HIST_TPC - 1) / HIST_TPC, n_cols), ANV_BLOCK, 0, st>>>(S);
-      sort_totals_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(S, sample_totals);
-      sort_scan_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(S, sample_totals);
-      sort_scatter_kernel<uint32_t><<<dim3((S.n_tiles + SCAT_TPC - 1) / SCAT_TPC, n_cols), SCAT_THREADS, 0, st>>>(S);
-      ANV_CUDA(cudaGetLastError());
-    }
+    if (int e = lsd_passes(S, sample_totals, 0, 4, st)) return e;
     pc_split_kernel<<<n_cols, 256, 0, st>>>(S, P);
     ANV_CUDA(cudaGetLastError());
   }
   if (n_rows > 0) {
     pc_coarse_kernel<<<dim3((L.n_tiles + PC_TPC - 1) / PC_TPC, n_cols), ANV_BLOCK, 0, st>>>(P);
-    sort_totals_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(T, P.totals);
-    sort_scan_kernel<uint32_t><<<dim3(256, n_cols), ANV_BLOCK, 0, st>>>(T, P.totals);
+    scan_tile_counts(T, P.totals, st);
     pc_chunks_kernel<<<n_cols, 256, 0, st>>>(P);
     pc_fine_kernel<<<dim3(L.max_chunks, n_cols), ANV_BLOCK, 0, st>>>(P);
     ANV_CUDA(cudaGetLastError());

@@ -555,9 +555,6 @@ def sort_mode_distinct(frame: ColumnFrame, names, ranks=None, hll_p=None):
             hregs[np.asarray(idxs)] = _host(dregs.view(torch.uint8)).view(np.uint32)[:n_all * hll_m].reshape(n_all, hll_m)
         del ws
         for j, i in enumerate(idxs):
-            if hr[j] == -3:
-                raise _lib.AnvError("anv_mode_distinct: a one-sweep look-back gave up waiting for a preceding tile (column %r); "
-                                    "unset ANV_SORT_ONESWEEP to use the three-kernel passes" % names[i])
             if n_ranks:
                 rvals[i] = hrv[j]
             if hr[j] <= 0:

@@ -52,10 +52,6 @@ FRIENDLY = [
     (r"sort_hist", "sort: tile digit histogram `sort_hist_kernel`"),
     (r"sort_totals", "sort: digit totals `sort_totals_kernel`"),
     (r"sort_scan", "sort: digit/tile scan `sort_scan_kernel`"),
-    (r"sort_onesweep", "sort: one-sweep scatter `sort_onesweep_kernel` (opt-in)"),
-    (r"sort_bases", "sort: digit bases `sort_bases_kernel` (opt-in one-sweep)"),
-    (r"pc_partition", "partition path: `pc_partition_kernel` (opt-in)"),
-    (r"pc_count", "partition path: `pc_count_kernel` (opt-in)"),
     (r"pc_", "partition path: small kernels (opt-in)"),
     (r"spark_sample", "Spark Bernoulli sampler `spark_sample_kernel`"),
     (r"sort_scatter", "sort: stable scatter `sort_scatter_kernel`"),

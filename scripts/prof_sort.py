@@ -31,10 +31,10 @@ hll_p = int(sys.argv[6]) if len(sys.argv) > 6 else anv_profile.DEFAULT_HLL_P
 with_ranks = (sys.argv[7] != "0") if len(sys.argv) > 7 else True
 engine.sort_algorithm = algo
 
-FAMILIES = ["pack_kernel", "sort_bases_kernel", "sort_hist_kernel", "sort_totals_kernel", "sort_scan_kernel",
-            "sort_scatter_kernel", "sort_onesweep_kernel", "run_tile_kernel", "run_merge_kernel",
+FAMILIES = ["pack_kernel", "sort_hist_kernel", "sort_totals_kernel", "sort_scan_kernel", "sort_scatter_kernel",
+            "run_tile_kernel", "run_merge_kernel",
             "pc_sample_kernel", "pc_split_kernel", "pc_coarse_kernel", "pc_chunks_kernel", "pc_fine_kernel", "pc_cum_kernel",
-            "pc_group_kernel", "pc_direct_kernel", "pc_final_kernel", "pc_partition_kernel", "pc_count_kernel"]
+            "pc_group_kernel", "pc_direct_kernel", "pc_final_kernel"]
 
 
 def family(name):

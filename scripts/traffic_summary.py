@@ -13,7 +13,7 @@ import re
 CALL_OF = [  # first match wins
     (r"pc_", "anv_mode_distinct_partition"),
     (r"pack_kernel|run_tile|run_merge", "anv_mode_distinct"),
-    (r"sort_hist|sort_totals|sort_scan|sort_scatter|sort_onesweep|sort_bases", "SORT"),      # LSD passes: the full sort, or the sample sort of the partition path
+    (r"sort_hist|sort_totals|sort_scan|sort_scatter", "SORT"),      # LSD passes: the full sort, or the sample sort of the partition path
     (r"hll_kernel", "anv_hll_registers"),
     (r"scan_kernel<\(bool\)1, \(int\)-1|scan_kernel<1, *\(?i?n?t?\)?-1|finalize_moments", "anv_moments"),
     (r"scan_kernel<\(bool\)1|scan_kernel<1", "anv_moments_hist"),

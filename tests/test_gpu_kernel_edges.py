@@ -495,14 +495,10 @@ def test_select_ranks_on_special_values(frame_kind):
         assert _same_float(got[i], exp[i]), (c, got[i], exp[i])
 
 
-@pytest.fixture(params=["lsd", "lsd-onesweep", "partition"])
-def sort_algo(request, monkeypatch):
+@pytest.fixture(params=["lsd", "partition"])
+def sort_algo(request):
     from anovos_b200 import engine
-    if request.param == "lsd-onesweep":
-        monkeypatch.setenv("ANV_SORT_ONESWEEP", "1")
-    else:
-        monkeypatch.delenv("ANV_SORT_ONESWEEP", raising=False)
-    old, engine.sort_algorithm = engine.sort_algorithm, request.param.split("-")[0]
+    old, engine.sort_algorithm = engine.sort_algorithm, request.param
     yield request.param
     engine.sort_algorithm = old
 

@@ -199,16 +199,12 @@ def test_select_ranks_exact(n):
     assert np.array_equal(got, np.array(exp), equal_nan=True)   # exact order statistics
 
 
-@pytest.fixture(params=["lsd", "lsd-onesweep", "partition"])
-def sort_algo(request, monkeypatch):
-    """Every implementation of the exact mode / distinct / order-statistic path: the LSD radix sort with its default
-    three-kernel passes, with the one-sweep passes (ANV_SORT_ONESWEEP=1, read per call), and the partition + count path."""
+@pytest.fixture(params=["lsd", "partition"])
+def sort_algo(request):
+    """Every implementation of the exact mode / distinct / order-statistic path: the LSD radix sort and the partition +
+    count path."""
     from anovos_b200 import engine
-    if request.param == "lsd-onesweep":
-        monkeypatch.setenv("ANV_SORT_ONESWEEP", "1")
-    else:
-        monkeypatch.delenv("ANV_SORT_ONESWEEP", raising=False)
-    old, engine.sort_algorithm = engine.sort_algorithm, request.param.split("-")[0]
+    old, engine.sort_algorithm = engine.sort_algorithm, request.param
     yield request.param
     engine.sort_algorithm = old
 
@@ -318,7 +314,7 @@ def test_moments_hist_without_early_pivot():
 
 
 @pytest.mark.parametrize("n", [300_007, 3_000_001])
-def test_partition_count_adversarial_columns(n, monkeypatch):
+def test_partition_count_adversarial_columns(n):
     """The partition + count path on the inputs that stress it: heavy hitters below and above the splitter threshold,
     discrete columns (every key equals a splitter), a constant column, an all-null column, NaN runs, keys on both sides of
     zero, near-constant columns with a few outliers, sorted input (the sample positions are stratified) - against NumPy,
@@ -357,16 +353,11 @@ def test_partition_count_adversarial_columns(n, monkeypatch):
         got, qv = engine.sort_mode_distinct(fr, names, rk)
         engine.sort_algorithm = "lsd"
         ref, qr = engine.sort_mode_distinct(fr, names, rk)
-        monkeypatch.setenv("ANV_SORT_ONESWEEP", "1")           # the one-sweep passes give the same sorted keys
-        one, q1 = engine.sort_mode_distinct(fr, names, rk)
-        monkeypatch.delenv("ANV_SORT_ONESWEEP")
     finally:
         engine.sort_algorithm = old
-    assert np.array_equal(q1, qr, equal_nan=True)
     def same(a, b):      # (mode, rows, distinct) tuples; the mode of a NaN-dominated column is NaN on both sides
         return a == b or (a[1:] == b[1:] and a[0] != a[0] and b[0] != b[0])
     assert all(same(a, b) for a, b in zip(got, ref)), [(n, a, b) for n, a, b in zip(names, got, ref) if not same(a, b)]
-    assert all(same(a, b) for a, b in zip(one, ref))
     assert np.array_equal(qv, qr, equal_nan=True)
     for i, c in enumerate(names):
         vals, valid = S.column_values(t, c)
