@@ -5,8 +5,10 @@ Both are a (group x label) contingency table per attribute.  The reference bins 
 attributes with the Python UDF of attribute_binning and then runs one groupBy per attribute;
 here the table comes from THREE runs of the histogram kernel (K2 / the code histogram) over
 the same columns with the validity bitmap AND-ed with the label-class bitmaps (all rows /
-event rows / non-event rows): no new kernel, bit-exact counts, then a few logs per group on
-the host.  `monotonicity_check=1` (monotonic_binning) is not part of this build."""
+event rows / non-event rows): bit-exact counts, then a few logs per group on the host.  With
+`monotonicity_check=1` the numeric attributes are binned as monotonic_binning bins them (:350-357), and their table comes
+from the same label-class histogram (anv_class_hist) that chose each attribute's bin count; only an attribute that falls
+back to a bin_size outside 3 .. 20 takes the three K2 passes."""
 from __future__ import annotations
 
 import math
@@ -60,32 +62,39 @@ def _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_conf
     if any(fr.column(c).kind == "other" for c in cols):
         raise TypeError("Invalid input for Column(s)")
     binned = bool(num) and bool(encoding_configs)
-    if binned and encoding_configs.get("monotonicity_check", 0) == 1:
-        raise NotImplementedError("monotonic_binning is outside the GPU hot-path build")
     return fr, cols, num, cat, ev_w, nev_w, binned
 
 
-def _contingency(fr, cols, num, cat, ev_w, nev_w, binned, encoding_configs):
+def _contingency(fr, cols, num, cat, ev_w, nev_w, binned, encoding_configs, label):
     """dict col -> (all[g], event[g], nonevent[g]) count arrays; index 0 = the null group."""
     out = {}
     if num and not binned:
         raise NotImplementedError("raw (unbinned) numeric attributes: pass encoding_configs")
-    views = {"all": fr, "ev": _masked(fr, cols, ev_w), "nev": _masked(fr, cols, nev_w)}
-    hists = {}
-    if num:
+
+    def views(names):                        # the class views of the columns a pass reads
+        return {"all": fr, "ev": _masked(fr, names, ev_w), "nev": _masked(fr, names, nev_w)}
+
+    hists = {"all": {}, "ev": {}, "nev": {}}
+    k2 = []                                  # (col, cutoffs, lohi) counted by K2 over the three views
+    if num and encoding_configs.get("monotonicity_check", 0) == 1:
+        k2 = _monotonic_groups(fr, num, encoding_configs, *label, hists)
+    elif num:
         kept, cuts, lohi = compute_cutoffs(getattr(fr, "_cut_source", fr), num, encoding_configs["bin_method"],
                                            encoding_configs["bin_size"])
-        for k, f in views.items():
-            model = engine.BinModel(f, kept, cuts, lohi)
-            h = engine.histogram(f, model)
-            hists[k] = {c: h[i, :len(cuts[i]) + 2].astype(np.int64) for i, c in enumerate(kept)}
+        k2 = list(zip(kept, cuts, lohi))
         for c in num:
-            if c not in hists["all"]:          # all-null attribute: only the null group exists
+            if c not in kept:                  # all-null attribute: only the null group exists
                 hists["all"][c] = hists["ev"][c] = hists["nev"][c] = None
+    if k2:
+        names = [c for c, _, _ in k2]
+        for k, f in views(names).items():
+            model = engine.BinModel(f, names, [cut for _, cut, _ in k2], [lh for _, _, lh in k2])
+            h = engine.histogram(f, model)
+            hists[k].update({c: h[i, :len(cut) + 2].astype(np.int64) for i, (c, cut, _) in enumerate(k2)})
     if cat:
-        for k, f in views.items():
+        for k, f in views(cat).items():
             cc = engine.code_counts(f, cat)
-            hists.setdefault(k, {}).update({c: h.astype(np.int64) for c, h in zip(cat, cc)})
+            hists[k].update({c: h.astype(np.int64) for c, h in zip(cat, cc)})
     n_rows = fr.n_rows
     tot_ev = int(_unpack_count(ev_w))
     tot_nev = int(_unpack_count(nev_w))
@@ -100,6 +109,24 @@ def _contingency(fr, cols, num, cat, ev_w, nev_w, binned, encoding_configs):
         ne[0] = tot_nev - ne[1:].sum()
         out[c] = (a, e, ne)
     return out, tot_ev, tot_nev
+
+
+def _monotonic_groups(fr, num, encoding_configs, label_col, event_label, hists):
+    """Fills hists["all" / "ev" / "nev"][col] for the numeric attributes binned as monotonic_binning bins them.  The groups
+    of an accepted n (or of a fallback bin_size inside 3 .. 20) are sums of the ladder's class histogram.  -> the
+    (col, cutoffs, lohi) of the columns that fall back to a bin_size outside that range, for the K2 passes."""
+    from ..data_transformer.transformers import monotonic_models
+    from ..shared import monotonic
+    models, lad = monotonic_models(getattr(fr, "_cut_source", fr), fr, num, label_col, event_label,
+                                   encoding_configs["bin_method"], encoding_configs["bin_size"])
+    rest = []
+    for c in num:
+        n, cut, lohi = models[c]
+        if n in lad[c].um.bins:
+            hists["all"][c], hists["ev"][c], hists["nev"][c] = monotonic.model_table(lad[c].um, lad[c].counts, n)
+        else:
+            rest.append((c, cut, lohi))
+    return rest
 
 
 def _unpack_count(words):
@@ -117,7 +144,8 @@ def IV_calculation(spark, idf, list_of_cols="all", drop_cols=[], label_col="labe
     """[attribute, iv]; iv = sum_g (nonevent_pcr - event_pcr) * woe_g with the reference's +0.5 smoothing
     when one side of a group is empty (:369-392)."""
     fr, cols, num, cat, ev_w, nev_w, binned = _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_configs)
-    tab, t1, t0 = _contingency(fr, cols, num, cat, ev_w, nev_w, binned, encoding_configs)
+    tab, t1, t0 = _contingency(fr, cols, num, cat, ev_w, nev_w, binned, encoding_configs,
+                               (label_col, event_label))
     rows = []
     for c in cols:
         a, e, ne = tab[c]
@@ -141,7 +169,8 @@ def IG_calculation(spark, idf, list_of_cols="all", drop_cols=[], label_col="labe
     """[attribute, ig]; ig = H(label) - sum_g segment_pct * H(label | g); log2(0) is NULL in Spark SQL, so a
     segment whose event_pct is 0 or 1 adds nothing (:540-566)."""
     fr, cols, num, cat, ev_w, nev_w, binned = _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_configs)
-    tab, t1, t0 = _contingency(fr, cols, num, cat, ev_w, nev_w, binned, encoding_configs)
+    tab, t1, t0 = _contingency(fr, cols, num, cat, ev_w, nev_w, binned, encoding_configs,
+                               (label_col, event_label))
     n = fr.n_rows
     te = t1 / n
     total_entropy = -(te * math.log2(te) + (1 - te) * math.log2(1 - te))

@@ -168,6 +168,74 @@ def attribute_binning(spark, idf, list_of_cols="all", drop_cols=[], method_type=
     return odf
 
 
+def monotonic_models(cut_fr, hist_fr, cols, label_col, event_label, bin_method, bin_size):
+    """-> ({col: (n, cutoffs, lohi)}, {col: Ladder}) of monotonic_binning: the first n of 20 .. 3 whose bins' event rate
+    rises with the bin (shared/monotonic.py), else bin_size.  Ladder cutoffs are reused; only a fallback bin_size outside
+    3 .. 20 computes its own."""
+    from ..shared import monotonic
+    lad = monotonic.ladders(cut_fr, hist_fr, cols, label_col, event_label, bin_method)
+    models = {}
+    for c in cols:
+        n = lad[c].n if lad[c].n is not None else bin_size
+        if n in lad[c].cuts:
+            models[c] = (n, lad[c].cuts[n], lad[c].lohi)
+    rest = [c for c in cols if c not in models]
+    if rest:
+        if bin_size < 2:
+            raise TypeError("Invalid input for bin_size")
+        kept, cuts, lohi = compute_cutoffs(cut_fr, rest, bin_method, bin_size)
+        models.update((c, (bin_size, cut, lh)) for c, cut, lh in zip(kept, cuts, lohi))
+    return models, lad
+
+
+def monotonic_binning(spark, idf, list_of_cols="all", drop_cols=[], label_col="label", event_label=1,
+                      bin_method="equal_range", bin_size=10, bin_dtype="numerical", output_mode="replace"):
+    """transformers.py:294-425.  Each numeric column is binned with the first bin count n = 20, 19, ..., 3 whose bins,
+    without the null group and bins averaging to NaN, have a Spearman correlation of exactly 1.0 between avg(x) and the
+    event rate (label == event_label; a null label counts as a non-event), and with bin_size when no n qualifies.  All
+    18 candidates of every column are counted in one pass (anv_class_hist).  Columns keep the input's order."""
+    fr = as_frame(idf)
+    if getattr(fr, "is_partitioned", False) and fr.group is not None:
+        raise NotImplementedError("monotonic_binning on row slabs of several ranks: repartition_to_columns first")
+    num_cols = attributeType_segregation(fr)[0]
+    if isinstance(list_of_cols, str) and list_of_cols == "all":
+        list_of_cols = num_cols
+    drop = _names(drop_cols) + [label_col]
+    cols = []
+    for c in _names(list_of_cols):
+        if c not in drop and c not in cols:
+            cols.append(c)
+    if any(c not in num_cols for c in cols):
+        raise TypeError("Invalid input for Column(s)")
+    if not cols:
+        return fr
+    if label_col not in fr.columns:
+        raise TypeError("Invalid input for Label Column")
+    if bin_method not in ("equal_frequency", "equal_range"):
+        raise TypeError("Invalid input for method_type")
+    if output_mode not in ("replace", "append"):
+        raise TypeError("Invalid input for output_mode")
+    models, _ = monotonic_models(fr, fr, cols, label_col, event_label, bin_method, bin_size)
+
+    # one bin_assign per bin count: _apply_binning's `len(cuts[0]) + 1` label quirk assumes one bin_size per call
+    odf = fr
+    for n in dict.fromkeys(models[c][0] for c in cols):
+        grp = [c for c in cols if models[c][0] == n]
+        cuts = [models[c][1] for c in grp]
+        lohi = [models[c][2] for c in grp]
+        if getattr(odf, "is_partitioned", False):
+            schema = _apply_binning(odf._schema, grp, cuts, lohi, bin_dtype, output_mode)
+            odf = odf.map_chunks(schema, lambda ch, g=grp, cu=cuts, lh=lohi: _apply_binning(ch, g, cu, lh, bin_dtype,
+                                                                                              output_mode))
+        else:
+            odf = _apply_binning(odf, grp, cuts, lohi, bin_dtype, output_mode)
+    if output_mode == "append":
+        order = list(fr.columns) + [c + "_binned" for c in cols]
+        if list(odf.columns) != order:
+            odf = odf.select(order)
+    return odf
+
+
 # ---- imputation_MMM (reference transformers.py:1369-1676) -------------------------------------------------------------
 #
 # Numeric columns under "mean" / "median" go through Spark ML's Imputer: statistics over the non-null, non-NaN values of

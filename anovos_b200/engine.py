@@ -1153,3 +1153,63 @@ def flag_members(frame: ColumnFrame, names, tables, want_bitmap):
     for j, i in enumerate(launch):
         counts[i] = flat[offs[j]:offs[j + 1]].copy()
     return counts, [None if v is None else v[:n_words] for v in valid]
+
+
+# ---- label-class histogram (monotonic_binning) ----------------------------------------------------
+
+_CLASS_HIST_SPEC_DT = np.dtype([("thresholds", "<u8"), ("n_thr", "<i4"), ("reserved", "<i4"), ("counts", "<u8")])
+
+
+def class_hist_counters(n_thr) -> int:
+    """Counters of one column of anv_class_hist: 3 label classes x (null, n_thr + 1 value slots, NaN), then -inf, +inf."""
+    return 3 * (int(n_thr) + 3) + 2
+
+
+def class_hist_max_thresholds() -> int:
+    return int(_lib.lib().anv_class_hist_max_thresholds())
+
+
+def class_hist(frame: ColumnFrame, names, thresholds, label_col, event_label):
+    """anv_class_hist: thresholds = per name, a host array of the column's own dtype holding distinct values in ascending
+    order (no NaN).  Rows are classed by label_col == event_label (event / non-event / null label, as
+    shared.label_classes.label_bitmaps does).  -> list of uint64 ndarrays [class_hist_counters(len(thresholds[i]))]:
+    [cls * (n_thr + 3) + slot] with slot 0 = null value, 1 + #(theta < x), n_thr + 2 = NaN; then the -inf and +inf
+    counts.  A row-partitioned frame is summed over its chunks."""
+    if getattr(frame, "is_partitioned", False):
+        return frame.class_hist(list(names), list(thresholds), label_col, event_label)
+    from .shared.label_classes import label_bitmaps
+    ev, nev, _ = label_bitmaps(frame, label_col, event_label)
+    return _class_hist_words(frame, list(names), list(thresholds), ev, nev)
+
+
+def _class_hist_words(frame, names, thresholds, ev_words, nev_words):
+    global launch_count
+    torch = _lib.require_cuda()
+    L = _lib.lib()
+    if len(names) > _lib.MAX_LAUNCH_COLS:
+        return _in_column_blocks(lambda lo, hi: _class_hist_words(frame, names[lo:hi], thresholds[lo:hi], ev_words,
+                                                                  nev_words), len(names))
+    max_thr = class_hist_max_thresholds()
+    thr = []
+    for n, t in zip(names, thresholds):
+        want = _NP_OF_ANV.get(frame.column(n).anv_dtype)
+        t = np.asarray(t)
+        if want is None or t.dtype != want or len(t) > max_thr or (t.dtype.kind == "f" and np.isnan(t).any()) \
+                or (len(t) > 1 and not bool(np.all(t[1:] > t[:-1]))):
+            raise ValueError("class_hist: column %r needs at most %d distinct ascending %s thresholds" % (n, max_thr, want))
+        thr.append(t)
+    offs = np.cumsum([0] + [class_hist_counters(len(t)) for t in thr])
+    if not names or not frame.n_rows:
+        return [np.zeros(int(offs[i + 1] - offs[i]), np.uint64) for i in range(len(names))]
+    dcounts = torch.zeros(int(offs[-1]), dtype=torch.int64, device="cuda")
+    buf, addr = _tables_to_dev(thr)
+    sp = np.zeros(len(names), _CLASS_HIST_SPEC_DT)
+    for i, t in enumerate(thr):
+        sp[i] = (addr[i], len(t), 0, dcounts.data_ptr() + 8 * int(offs[i]))
+    desc, keep = frame.descriptors(names)
+    dspecs = _to_dev(sp)                                # held until the launch is enqueued
+    _call(L.anv_class_hist, "anv_class_hist", desc.data_ptr(), dspecs.data_ptr(), ev_words.data_ptr(), nev_words.data_ptr(),
+          len(names), frame.n_rows, _stream(), nbytes=input_bytes(frame, names))
+    launch_count += 1
+    flat = _host(dcounts).view(np.uint64)
+    return [flat[offs[i]:offs[i + 1]].copy() for i in range(len(names))]

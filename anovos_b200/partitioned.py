@@ -326,6 +326,16 @@ class PartitionedFrame:
             acc = [flat[offs[i]:offs[i + 1]].copy() for i in range(len(acc))]
         return acc
 
+    def class_hist(self, names, thresholds, label_col, event_label):
+        """engine.class_hist summed over the chunks (each chunk classes its rows with its own slice of the label)."""
+        from . import engine
+        if self.group is not None:
+            raise NotImplementedError("class_hist on row slabs of several ranks: repartition_to_columns first")
+        acc = [np.zeros(engine.class_hist_counters(len(t)), np.uint64) for t in thresholds]
+        for ch in self.chunks(list(dict.fromkeys(list(names) + [label_col]))):
+            acc = [a + c for a, c in zip(acc, engine.class_hist(ch, names, thresholds, label_col, event_label))]
+        return acc
+
     def hll_registers(self, names, p):
         from . import engine
         names = list(names)

@@ -431,6 +431,26 @@ typedef struct {
 int anv_flag_members(const anv_column_t* cols, const anv_flag_spec_t* specs, int n_cols, int64_t n_rows, void* stream);
 int anv_flag_members_smem_keys(void);
 
+/* ---- label-class histogram (monotonic_binning, data_transformer/transformers.py:294-425).
+ * anv_class_hist: thresholds [dev] n_thr distinct native thresholds in ascending order (int32 / float for ANV_I32 / ANV_F32
+ * columns, int64 / double for ANV_I64 / ANV_F64 ones, no NaN), 0 <= n_thr <= anv_class_hist_max_thresholds().  Each row
+ * adds 1 to counts[cls * (n_thr + 3) + slot]: slot 0 for a null value, n_thr + 2 for NaN, 1 + #(theta < x) otherwise;
+ * cls 0 when the row's bit is set in event_words, 1 when it is set in nonevent_words, 2 when in neither (a null label).
+ * counts[3 * (n_thr + 3)] and counts[3 * (n_thr + 3) + 1] count the valid -inf and +inf values.  counts [dev]
+ * ANV_CLASS_HIST_COUNTERS(n_thr) uint64, zeroed by the caller (the pass adds to them).  event_words / nonevent_words [dev]
+ * ceil(n_rows/32) disjoint bitmaps.  A spec outside these rules leaves its counts untouched.  specs [dev] n_cols,
+ * n_cols <= ANV_MAX_LAUNCH_COLS. */
+#define ANV_CLASS_HIST_COUNTERS(n_thr) (3 * ((n_thr) + 3) + 2)
+typedef struct {
+  const void* thresholds;        /* [dev] n_thr ascending native thresholds */
+  int32_t n_thr;
+  int32_t reserved;
+  unsigned long long* counts;    /* [dev] ANV_CLASS_HIST_COUNTERS(n_thr) counts */
+} anv_class_hist_spec_t;
+int anv_class_hist(const anv_column_t* cols, const anv_class_hist_spec_t* specs, const uint32_t* event_words,
+                   const uint32_t* nonevent_words, int n_cols, int64_t n_rows, void* stream);
+int anv_class_hist_max_thresholds(void);
+
 /* ---- Spark's Bernoulli row sampler (the DEFAULT path of drift_detector.statistics: use_sampling=True ->
  *      data_sampling.py:122-149 `idf.sample(False, fraction, seed)` / `stat.sampleBy("merge", fractions, seed)`,
  *      drift_detector.py:187-211).  One partition per call: Spark seeds XORShiftRandom with seed + partitionIndex,
