@@ -968,6 +968,7 @@ struct PcParams {
   uint32_t* totals;                // [n_cols][256]           keys per group
   uint32_t* gstart;                // [n_cols][G + 1]         group-major offset of each group (+ the total)
   uint32_t* chunk_base;            // [n_cols][G + 1]         first fine chunk of each group (+ the total)
+  uint32_t* chunk_tile;            // [n_cols][max_chunks]    tile whose segment holds each chunk's first key << 8 | its group
   uint16_t* cst;                   // [n_cols][PC_CST][max_chunks]  bucket starts inside each chunk's range, bucket-major
   uint32_t* cnt_lt;                // [n_cols][NB]  keys strictly between two splitters, per bucket
   uint32_t* cnt_eq;                // [n_cols][NS]  keys equal to each splitter (the zero run is added by pc_cum_kernel)
@@ -1052,31 +1053,38 @@ __global__ void __launch_bounds__(256) pc_split_kernel(const SortParams<uint32_t
 }
 
 // ---- coarse: raw column -> keys grouped by coarse group inside each tile ------------------------------------------------
-template <typename T>
-__device__ __forceinline__ void pc_coarse_tile(const PcParams& P, const anv_column_t& col, const int c, const int64_t tile,
-                                               const uint32_t* sC, const uint16_t* sL, uint32_t* hc, uint32_t* s_warp, uint32_t* sk,
-                                               uint32_t& n_zero, uint32_t& n_keys) {
-  constexpr int PER = SORT_TILE / ANV_BLOCK;        // 16 rounds of 256 rows (the strided pack: coalesced scalar loads)
+constexpr int PC_QPT = SORT_TILE / 4 / ANV_BLOCK;   // quads of 4 rows per thread and tile
+
+// Thread tid ranks rows 4 q .. 4 q + 3 of quads q = tid + r * ANV_BLOCK (the order inside a group is free, so is the
+// row -> thread map), loaded as 128-bit words.  The tile's (group, tile) counts and starts go to column t of sH.
+__device__ __forceinline__ void pc_coarse_tile(const PcParams& P, const anv_column_t& col, const int c, const int64_t tile, const int t,
+                                               const uint32_t* sC, const uint16_t* sL, uint32_t* hc, uint32_t* s_warp,
+                                               uint32_t* sk, uint16_t (*sH)[PC_TPC], uint32_t& n_zero, uint32_t& n_keys) {
+  constexpr int PER = SORT_TILE / ANV_BLOCK;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t r0 = tile * SORT_TILE;              // multiple of 4096: the tile starts on a bitmap word
   const int n_tile = (int)min((int64_t)SORT_TILE, P.n_rows - r0);
-  const T* __restrict__ data = reinterpret_cast<const T*>(col.data) + r0 + tid;
-  const uint32_t* __restrict__ vw = col.validity ? col.validity + (r0 >> 5) + warp : nullptr;
-  const bool full = n_tile == SORT_TILE;
-  uint32_t wv = ANV_FULL;                           // lane i holds the warp's bitmap word of round i
-  if (vw && lane < PER && (full || lane * ANV_BLOCK + warp * 32 < n_tile)) wv = __ldg(vw + lane * (ANV_BLOCK / 32));
-  T x[PER];
+  const uint32_t* __restrict__ data = reinterpret_cast<const uint32_t*>(col.data) + r0;   // 16-byte aligned
+  uint32_t key[PER], vb[PC_QPT];
 #pragma unroll
-  for (int i = 0; i < PER; ++i) {
-    const bool in = full || (i * ANV_BLOCK + tid) < n_tile;
-    x[i] = in ? ld_stream_scalar<T>(data + i * ANV_BLOCK) : (T)0;
+  for (int r = 0; r < PC_QPT; ++r) {
+    const int q = tid + r * ANV_BLOCK;
+    vb[r] = col.validity && 4 * q < n_tile ? __ldg(col.validity + (r0 >> 5) + (q >> 3)) >> (4 * (q & 7)) : 0xFu;
+    if (4 * q + 4 <= n_tile) {
+      const uint4 v = ldg_stream(data + 4 * q);
+      key[4 * r] = v.x; key[4 * r + 1] = v.y; key[4 * r + 2] = v.z; key[4 * r + 3] = v.w;
+    } else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) key[4 * r + e] = 4 * q + e < n_tile ? data[4 * q + e] : 0u;
+    }
   }
-  uint32_t key[PER], slot[PER];                     // slot: group << 16 | rank inside the group, ~0 = no key
+  const bool f32 = col.dtype == ANV_F32;
+  uint32_t slot[PER];                               // group << 16 | rank inside the group, ~0 = no key
 #pragma unroll
   for (int i = 0; i < PER; ++i) {
-    const uint32_t k = make_key<uint32_t, T>(x[i]);
-    bool ok = (__shfl_sync(ANV_FULL, wv, i) >> lane) & 1u;
-    if (!full) ok = ok && (i * ANV_BLOCK + tid) < n_tile;
+    const int row = 4 * (tid + (i >> 2) * ANV_BLOCK) + (i & 3);
+    const uint32_t k = f32 ? make_key<uint32_t, float>(__uint_as_float(key[i])) : make_key<uint32_t, int32_t>((int32_t)key[i]);
+    bool ok = ((vb[i >> 2] >> (i & 3)) & 1u) && row < n_tile;
     const bool zero = ok && k == PC_ZERO_KEY;      // 0.0 and -0.0 share one key; integers: 0
     n_zero += zero ? 1u : 0u;
     ok = ok && !zero;
@@ -1101,27 +1109,37 @@ __device__ __forceinline__ void pc_coarse_tile(const PcParams& P, const anv_colu
 #pragma unroll
   for (int w = 0; w < ANV_WARPS; ++w) { const uint32_t t = s_warp[w]; woff += (w < warp) ? t : 0u; total += t; }
   const uint32_t start = woff + inc - cnt;
-  const size_t row = ((size_t)c * 256 + tid) * P.n_tiles + tile;
-  P.tile_hist[row] = cnt;
-  P.tile_start[row] = (uint16_t)start;
+  sH[tid][t] = (uint16_t)cnt;                       // <= 4096
+  sH[256 + tid][t] = (uint16_t)start;
   hc[tid] = start;                                  // every thread read its own count above and nothing else
   __syncthreads();
 #pragma unroll
   for (int i = 0; i < PER; ++i)
     if (slot[i] != ~0u) sk[hc[slot[i] >> 16] + (slot[i] & 0xFFFFu)] = key[i];
   __syncthreads();
+  // the output starts 16-byte aligned (stride is a multiple of 64 keys, r0 of 4096): whole uint4 stores, scalar tail
   uint32_t* __restrict__ out = P.keys[0] + (size_t)c * P.stride + r0;
-  for (uint32_t i = tid; i < total; i += ANV_BLOCK) out[i] = sk[i];
+#pragma unroll
+  for (int r = 0; r < PC_QPT; ++r) {
+    const uint32_t i = tid + r * ANV_BLOCK;
+    if (i < total / 4) reinterpret_cast<uint4*>(out)[i] = reinterpret_cast<const uint4*>(sk)[i];
+  }
+  if (tid < (total & 3u)) out[(total & ~3u) + tid] = sk[(total & ~3u) + tid];
   if (tid == 0) n_keys += total;
   hc[tid] = 0;
   __syncthreads();                                  // sk / hc / s_warp are reused by the CTA's next tile
 }
 
+// The (group, tile) counts and starts of the CTA's PC_TPC tiles are kept in shared memory and written at its end, PC_TPC
+// adjacent entries per group row.  Written per tile they are 512 lone 2- and 4-byte stores into 512 rows, partial-sector
+// writes that the rest of the sector joins only tiles later; at c3 on H100 (700 W) writing them per CTA took the pass
+// from 34 to 29 ms.
 __global__ void __launch_bounds__(ANV_BLOCK, 4) pc_coarse_kernel(const PcParams P) {
   __shared__ uint32_t sC[PC_MAX_P / PC_FPG];
   __shared__ uint16_t sL[PC_LUT_CELLS + 1];
   __shared__ uint32_t hc[256], s_warp[ANV_WARPS];
-  __shared__ uint32_t sk[SORT_TILE];
+  __shared__ __align__(16) uint32_t sk[SORT_TILE];
+  __shared__ uint16_t sH[2 * 256][PC_TPC];           // [group] counts, then [256 + group] starts, per tile of the CTA
   const int c = blockIdx.y, tid = threadIdx.x;
   const anv_column_t col = P.cols[c];
   const uint32_t* S = P.split + (size_t)c * P.NS;
@@ -1130,12 +1148,18 @@ __global__ void __launch_bounds__(ANV_BLOCK, 4) pc_coarse_kernel(const PcParams 
   for (int i = tid; i <= PC_LUT_CELLS; i += ANV_BLOCK) sL[i] = L[i];
   hc[tid] = 0;
   __syncthreads();
+  const int64_t t_first = (int64_t)blockIdx.x * PC_TPC;
+  const int n_t = (int)min((int64_t)PC_TPC, P.n_tiles - t_first);
   uint32_t n_zero = 0, n_keys = 0;
-  for (int t = 0; t < PC_TPC; ++t) {
-    const int64_t tile = (int64_t)blockIdx.x * PC_TPC + t;
-    if (tile >= P.n_tiles) break;
-    if (col.dtype == ANV_F32) pc_coarse_tile<float>(P, col, c, tile, sC, sL, hc, s_warp, sk, n_zero, n_keys);
-    else pc_coarse_tile<int32_t>(P, col, c, tile, sC, sL, hc, s_warp, sk, n_zero, n_keys);
+  for (int t = 0; t < n_t; ++t) pc_coarse_tile(P, col, c, t_first + t, t, sC, sL, hc, s_warp, sk, sH, n_zero, n_keys);
+#pragma unroll
+  for (int r = 0; r < 256 * PC_TPC / ANV_BLOCK; ++r) {   // thread -> (group, tile): a group's tiles are adjacent
+    const int i = tid + r * ANV_BLOCK, g = i / PC_TPC, t = i % PC_TPC;
+    if (t < n_t) {
+      const size_t row = ((size_t)c * 256 + g) * P.n_tiles + t_first + t;
+      P.tile_hist[row] = sH[g][t];
+      P.tile_start[row] = sH[256 + g][t];
+    }
   }
   n_zero = __reduce_add_sync(ANV_FULL, n_zero);
   if ((tid & 31) == 0 && n_zero) atomicAdd(&P.state[c].n_zero, (unsigned long long)n_zero);
@@ -1165,6 +1189,20 @@ __global__ void __launch_bounds__(256) pc_chunks_kernel(const PcParams P) {
   if (tid == 0) { gs[P.G] = tt; cb[P.G] = tk; }
 }
 
+// ---- the tile that holds each fine chunk's first key: one walk over each group's scanned (group, tile) row ---------------
+__global__ void __launch_bounds__(ANV_BLOCK) pc_chunk_tiles_kernel(const PcParams P) {
+  const int g = blockIdx.x, c = blockIdx.y;
+  const uint32_t* gs = P.gstart + (size_t)c * (P.G + 1);
+  const uint32_t g0 = gs[g], gend = gs[g + 1];
+  const uint32_t* O = P.tile_hist + ((size_t)c * 256 + g) * P.n_tiles;
+  uint32_t* ct = P.chunk_tile + (size_t)c * P.max_chunks + P.chunk_base[(size_t)c * (P.G + 1) + g];
+  for (int t = threadIdx.x; t < P.n_tiles; t += ANV_BLOCK) {
+    const uint32_t lo = O[t] - g0, hi = (t + 1 < P.n_tiles ? O[t + 1] : gend) - g0;   // the segment, relative to the group
+    // chunk k starts at k * PC_CHUNK (n_tiles < 2^20, so t << 8 | g fits)
+    for (uint32_t k = lo / PC_CHUNK + (lo % PC_CHUNK != 0u); (uint64_t)k * PC_CHUNK < hi; ++k) ct[k] = (uint32_t)t << 8 | g;
+  }
+}
+
 // 4-byte cp.async copies into shared memory: a thread issues all of its copies before it waits for any
 __device__ __forceinline__ void pc_cp_async4(uint32_t* dst, const uint32_t* src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
@@ -1184,66 +1222,81 @@ __device__ __forceinline__ uint32_t pc_fine_bucket(const uint32_t* sF, uint32_t 
 
 // ---- fine: one CTA per chunk of <= 4096 group-major keys -------------------------------------------------------------
 __global__ void __launch_bounds__(ANV_BLOCK) pc_fine_kernel(const PcParams P) {
-  const int c = blockIdx.y, b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int c = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t b = blockIdx.x;
   const uint32_t* cb = P.chunk_base + (size_t)c * (P.G + 1);
-  if ((uint32_t)b >= cb[P.G]) return;               // (uniform) the grid is sized for the largest possible chunk count
-  __shared__ uint32_t sk[PC_CHUNK], sk2[PC_CHUNK];
+  if (b >= cb[P.G]) return;                         // (uniform) the grid is sized for the largest possible chunk count
+  __shared__ __align__(16) uint32_t sk[PC_CHUNK], sk2[PC_CHUNK];
   __shared__ uint32_t sO[PC_WIN + 1];
   __shared__ uint16_t sTS[PC_WIN];
   __shared__ uint32_t sF[PC_FPG], lc[PC_FPG + 1], ec[PC_FPG], ls[PC_CST];
-  __shared__ int s_g, s_t0;
+  __shared__ uint32_t s_wmax[ANV_WARPS];
+  uint16_t* sSeg = reinterpret_cast<uint16_t*>(sk2);   // gather: window segment of each chunk position (sk2 is free till ranked)
   const uint32_t* gs = P.gstart + (size_t)c * (P.G + 1);
-  if (warp == 0) {
-    int g = 0;
-    if (lane == 0) {                                // the group owning chunk b: last g with cb[g] <= b
-      int lo = 0, hi = P.G;
-      while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (cb[mid] <= (uint32_t)b) lo = mid; else hi = mid - 1; }
-      g = lo;
-    }
-    g = __shfl_sync(ANV_FULL, g, 0);
-    const uint32_t p0 = gs[g] + ((uint32_t)b - cb[g]) * PC_CHUNK;
-    // the tile whose segment holds p0: last t with O[t] <= p0, 32-ary search (O is non-decreasing over the tiles)
-    const uint32_t* O = P.tile_hist + ((size_t)c * 256 + g) * P.n_tiles;
-    int lo = 0, hi = P.n_tiles;
-    while (hi - lo > 1) {
-      const int step = (hi - lo + 31) / 32;
-      const int idx = lo + lane * step;
-      const uint32_t bal = __ballot_sync(ANV_FULL, idx < hi && O[idx] <= p0);   // lane 0 always: O[lo] <= p0
-      lo += (31 - __clz(bal)) * step;
-      hi = min(hi, lo + step);
-    }
-    if (lane == 0) { s_g = g; s_t0 = lo; }
-  }
-  if (tid < PC_FPG) ec[tid] = 0;
-  if (tid <= PC_FPG) lc[tid] = 0;
-  __syncthreads();
-  const int g = s_g;
+  const uint32_t ct = P.chunk_tile[(size_t)c * P.max_chunks + b];
+  const int g = ct & 0xFFu;
   const uint32_t gend = gs[g + 1];
-  const uint32_t p0 = gs[g] + ((uint32_t)b - cb[g]) * PC_CHUNK;
+  const uint32_t p0 = gs[g] + (b - cb[g]) * PC_CHUNK;
   const uint32_t p1 = p0 + min((uint32_t)PC_CHUNK, gend - p0);   // p0 + PC_CHUNK may pass 2^32 in a column of < 2^32 keys
   const uint32_t* O = P.tile_hist + ((size_t)c * 256 + g) * P.n_tiles;
   const uint16_t* TS = P.tile_start + ((size_t)c * 256 + g) * P.n_tiles;
   const uint32_t* __restrict__ src = P.keys[0] + (size_t)c * P.stride;
-  if (tid < PC_FPG) sF[tid] = P.split[(size_t)c * P.NS + g * PC_FPG + tid];
-  // gather: the chunk's keys are the segments of consecutive tiles, in tile order; a round locates PC_WIN of them
-  for (int t0 = s_t0;; t0 += PC_WIN) {
-    for (int i = tid; i <= PC_WIN; i += ANV_BLOCK) {
-      const int t = t0 + i;
-      sO[i] = t < P.n_tiles ? O[t] : gend;
+  if (tid < PC_FPG) { ec[tid] = 0; sF[tid] = P.split[(size_t)c * P.NS + g * PC_FPG + tid]; }
+  if (tid <= PC_FPG) lc[tid] = 0;
+  // gather: the chunk's keys are the segments of consecutive tiles, in tile order; a round covers PC_WIN of them.  Each
+  // non-empty segment marks its first chunk position with its window index, and a block max-scan gives every position
+  // its segment, so no key searches for it.
+  constexpr int SPT = PC_CHUNK / ANV_BLOCK;         // chunk positions per thread in the scan
+  static_assert(SPT == 16 && PC_WIN <= 65536, "the scan moves a thread's 16 uint16 segment indices as two uint4");
+  for (int t0 = (int)(ct >> 8);; t0 += PC_WIN) {
+#pragma unroll
+    for (int r = 0; r <= PC_WIN / ANV_BLOCK; ++r) {  // fixed trip counts: nvcc emits no remainder loops
+      const int i = tid + r * ANV_BLOCK, t = t0 + i;
+      if (i <= PC_WIN) sO[i] = t < P.n_tiles ? O[t] : gend;
       if (i < PC_WIN && t < P.n_tiles) sTS[i] = TS[t];
     }
+    uint4* seg4 = reinterpret_cast<uint4*>(sSeg) + 2 * tid;
+    seg4[0] = seg4[1] = make_uint4(0u, 0u, 0u, 0u);
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < PC_WIN / ANV_BLOCK; ++r) {
+      const int i = tid + r * ANV_BLOCK;
+      const uint32_t a = sO[i], e = sO[i + 1];
+      if (a < e && a < p1 && e > p0) sSeg[max(a, p0) - p0] = (uint16_t)i;
+    }
+    __syncthreads();
+    uint4 v[2] = {seg4[0], seg4[1]};
+    uint32_t* w = reinterpret_cast<uint32_t*>(v);
+    uint32_t run = 0;                               // segment indices rise with the position: a running max, in both halves
+#pragma unroll
+    for (int j = 0; j < SPT / 2; ++j) {
+      uint32_t x = __vmaxu2(w[j], run);
+      x = __vmaxu2(x, x << 16);                     // the upper position also takes the lower one's segment
+      w[j] = x;
+      run = __byte_perm(x, 0u, 0x3232);
+    }
+    uint32_t inc = run;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) inc = max(inc, __shfl_up_sync(ANV_FULL, inc, o));
+    if (lane == 31) s_wmax[warp] = inc;
+    uint32_t before = __shfl_up_sync(ANV_FULL, inc, 1);
+    if (lane == 0) before = 0;
+    __syncthreads();
+    before = max(before, __reduce_max_sync(ANV_FULL, lane < warp ? s_wmax[lane] : 0u));
+#pragma unroll
+    for (int j = 0; j < SPT / 2; ++j) w[j] = __vmaxu2(w[j], before);
+    seg4[0] = v[0];
+    seg4[1] = v[1];
     __syncthreads();
     const uint32_t wlo = max(p0, sO[0]), whi = min(p1, sO[PC_WIN]);
     // positions relative to p0 (< PC_CHUNK): q += ANV_BLOCK could wrap past 2^32 near the end of a long column
     const uint32_t i1 = whi > p0 ? whi - p0 : 0u;
     for (uint32_t i = wlo - p0 + tid; i < i1; i += ANV_BLOCK) {
-      const uint32_t q = p0 + i;
-      int lo = 0, hi = PC_WIN - 1;                  // last i with sO[i] <= q
-      while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (sO[mid] <= q) lo = mid; else hi = mid - 1; }
-      pc_cp_async4(&sk[i], src + (size_t)(t0 + lo) * SORT_TILE + sTS[lo] + (q - sO[lo]));   // nothing waits for it
+      const int s = sSeg[i];
+      pc_cp_async4(&sk[i], src + (size_t)(t0 + s) * SORT_TILE + sTS[s] + (p0 + i - sO[s]));   // nothing waits for it
     }
     const bool done = whi >= p1;
-    __syncthreads();                                // sO / sTS are refilled by the next round
+    __syncthreads();                                // sO / sTS / sSeg are refilled by the next round
     if (done) break;
   }
   pc_cp_commit();
@@ -1800,7 +1853,8 @@ __global__ void pc_final_kernel(const PcParams P, double* mode_value, int64_t* m
 struct PcLayout {
   int P, NS, NB, G, n_tiles, max_chunks;
   int64_t m, stride;
-  size_t state, split, clut, cnt_lt, cnt_eq, cum, st, totals, gstart, chunk_base, lsd, keys0, keys1, tile_hist, tile_start, cst, total;
+  size_t state, split, clut, cnt_lt, cnt_eq, cum, st, totals, gstart, chunk_base, lsd, keys0, keys1, tile_hist, tile_start, cst,
+      chunk_tile, total;
   PcLayout(int n_cols, int64_t n_rows) {
     int p = 256;                                   // fine buckets of ~4096 rows
     while (p < PC_MAX_P && (int64_t)p * SORT_TILE < n_rows) p <<= 1;
@@ -1830,6 +1884,7 @@ struct PcLayout {
     tile_hist = take((size_t)n_cols * 256 * n_tiles * 4);
     tile_start = take((size_t)n_cols * 256 * n_tiles * 2);
     cst = take((size_t)n_cols * max_chunks * PC_CST * 2);
+    chunk_tile = take((size_t)n_cols * max_chunks * 4);
     const size_t sample_end = lsd + Layout<uint32_t>(n_cols, m).total;
     total = (o > sample_end ? o : sample_end) + 256;
   }
@@ -1859,6 +1914,7 @@ static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_r
   P.gstart = reinterpret_cast<uint32_t*>(w + L.gstart);
   P.chunk_base = reinterpret_cast<uint32_t*>(w + L.chunk_base);
   P.cst = reinterpret_cast<uint16_t*>(w + L.cst);
+  P.chunk_tile = reinterpret_cast<uint32_t*>(w + L.chunk_tile);
   P.cnt_lt = reinterpret_cast<uint32_t*>(w + L.cnt_lt);
   P.cnt_eq = reinterpret_cast<uint32_t*>(w + L.cnt_eq);
   P.cum = reinterpret_cast<uint32_t*>(w + L.cum);
@@ -1885,6 +1941,7 @@ static int run_partition_count(const anv_column_t* cols, int n_cols, int64_t n_r
     pc_coarse_kernel<<<dim3((L.n_tiles + PC_TPC - 1) / PC_TPC, n_cols), ANV_BLOCK, 0, st>>>(P);
     scan_tile_counts(T, P.totals, st);
     pc_chunks_kernel<<<n_cols, 256, 0, st>>>(P);
+    pc_chunk_tiles_kernel<<<dim3(L.G, n_cols), ANV_BLOCK, 0, st>>>(P);
     pc_fine_kernel<<<dim3(L.max_chunks, n_cols), ANV_BLOCK, 0, st>>>(P);
     ANV_CUDA(cudaGetLastError());
   }

@@ -33,8 +33,8 @@ engine.sort_algorithm = algo
 
 FAMILIES = ["pack_kernel", "sort_hist_kernel", "sort_totals_kernel", "sort_scan_kernel", "sort_scatter_kernel",
             "run_tile_kernel", "run_merge_kernel",
-            "pc_sample_kernel", "pc_split_kernel", "pc_coarse_kernel", "pc_chunks_kernel", "pc_fine_kernel", "pc_cum_kernel",
-            "pc_group_kernel", "pc_direct_kernel", "pc_final_kernel"]
+            "pc_sample_kernel", "pc_split_kernel", "pc_coarse_kernel", "pc_chunks_kernel", "pc_chunk_tiles_kernel",
+            "pc_fine_kernel", "pc_cum_kernel", "pc_group_kernel", "pc_direct_kernel", "pc_final_kernel"]
 
 
 def family(name):
