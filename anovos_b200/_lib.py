@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("ANOVOS_B200_LIB") or os.path.join(HERE, "libanovos_b2
 
 ANV_F32, ANV_F64, ANV_I32, ANV_I64 = 0, 1, 2, 3
 MAX_LAUNCH_COLS = 65535   # ANV_MAX_LAUNCH_COLS of the header: columns per call of an entry point taking descriptors
+MAX_BINS = 16384          # ANV_MAX_BINS of the header: bins per column of anv_hist / anv_moments_hist / anv_bin_assign
 
 
 class AnvColumn(C.Structure):

@@ -116,7 +116,10 @@ extern "C" int anv_hist(const anv_column_t* cols, const anv_binspec_t* specs, co
   if (int e = check_common(cols, n_cols, n_rows)) return e;
   if (n_cols == 0) return ANV_OK;
   if (!specs || !counts || count_stride < 2) { set_error("anv_hist: bad specs/counts/count_stride"); return ANV_ERR_INVALID; }
-  if (count_stride > 16385) { set_error("anv_hist: more than 16384 bins per column is not supported"); return ANV_ERR_UNSUPPORTED; }
+  if (count_stride > ANV_MAX_BINS + 1) {
+    set_error("anv_hist: more than %d bins per column is not supported", ANV_MAX_BINS);
+    return ANV_ERR_UNSUPPORTED;
+  }
   cudaStream_t st = (cudaStream_t)stream;
   ANV_CUDA(cudaMemsetAsync(counts, 0, (size_t)n_cols * count_stride * sizeof(uint64_t), st));
   ScanParams P{};
@@ -150,7 +153,10 @@ extern "C" int anv_moments_hist(const anv_column_t* cols, const anv_binspec_t* s
   if (int e = check_common(cols, n_cols, n_rows)) return e;
   if (n_cols == 0) return ANV_OK;
   if (!specs || !counts || !out || count_stride < 2) { set_error("anv_moments_hist: bad arguments"); return ANV_ERR_INVALID; }
-  if (count_stride > 16385) { set_error("anv_moments_hist: more than 16384 bins per column is not supported"); return ANV_ERR_UNSUPPORTED; }
+  if (count_stride > ANV_MAX_BINS + 1) {
+    set_error("anv_moments_hist: more than %d bins per column is not supported", ANV_MAX_BINS);
+    return ANV_ERR_UNSUPPORTED;
+  }
   if (workspace_bytes < anv_moments_workspace_bytes(n_cols, n_rows) || !workspace) {
     set_error("anv_moments_hist: workspace too small");
     return ANV_ERR_WORKSPACE;
@@ -179,9 +185,13 @@ extern "C" int anv_bin_assign(const anv_column_t* cols, const anv_binspec_t* spe
                               int64_t n_rows, int max_bins, int32_t* out_bins, int64_t out_stride, void* stream) {
   if (int e = check_common(cols, n_cols, n_rows)) return e;
   if (n_cols == 0) return ANV_OK;
-  if (!specs || !out_bins || out_stride < n_rows || (out_stride & 3) || max_bins < 2 || max_bins > 4096) {
-    set_error("anv_bin_assign: bad arguments (out_stride must be >= n_rows and a multiple of 4; 2 <= max_bins <= 4096)");
+  if (!specs || !out_bins || out_stride < n_rows || (out_stride & 3) || max_bins < 2) {
+    set_error("anv_bin_assign: bad arguments (out_stride must be >= n_rows and a multiple of 4; max_bins >= 2)");
     return ANV_ERR_INVALID;
+  }
+  if (max_bins > ANV_MAX_BINS) {
+    set_error("anv_bin_assign: more than %d bins per column is not supported", ANV_MAX_BINS);
+    return ANV_ERR_UNSUPPORTED;
   }
   cudaStream_t st = (cudaStream_t)stream;
   ScanParams P{};

@@ -17,7 +17,7 @@ import numpy as np
 import pandas as pd
 
 from .. import engine
-from ..data_transformer.transformers import compute_cutoffs
+from ..data_transformer.transformers import check_bin_size, compute_cutoffs
 from ..frame import as_frame
 from ..result import ResultFrame
 from ..shared.label_classes import label_bitmaps as _label_bitmaps, masked as _masked
@@ -33,6 +33,8 @@ def _names(x):
 
 
 def _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_configs):
+    if encoding_configs and "bin_size" in encoding_configs:
+        check_bin_size(encoding_configs["bin_size"])
     fr = as_frame(idf)
     if getattr(fr, "is_partitioned", False):
         # chunked / Spark-partitioned table: the cutoffs come from the partitioned frame (so approxQuantile follows Spark's

@@ -54,6 +54,13 @@ def load_binning_model(model_path):
     return OrderedDict(zip(t.column("attribute").to_pylist(), t.column("parameters").to_pylist()))
 
 
+def check_bin_size(bin_size):
+    """Refuse a bin_size above the binning kernels' limit before any device work (the reference has no upper bound: a
+    deviation, DESIGN.md section 1)."""
+    if bin_size > _lib.MAX_BINS:
+        raise ValueError("bin_size %r: at most %d bins per column are supported" % (bin_size, _lib.MAX_BINS))
+
+
 def compute_cutoffs(fr: ColumnFrame, cols, method_type, bin_size):
     """-> (kept cols, cutoffs, (min,max) per kept col | None).  transformers.py:210-240."""
     mom = profile.moments(fr, cols)
@@ -137,6 +144,7 @@ def attribute_binning(spark, idf, list_of_cols="all", drop_cols=[], method_type=
         raise TypeError("Invalid input for method_type")
     if bin_size < 2:
         raise TypeError("Invalid input for bin_size")
+    check_bin_size(bin_size)
     if output_mode not in ("replace", "append"):
         raise TypeError("Invalid input for output_mode")
 
@@ -215,6 +223,7 @@ def monotonic_binning(spark, idf, list_of_cols="all", drop_cols=[], label_col="l
         raise TypeError("Invalid input for method_type")
     if output_mode not in ("replace", "append"):
         raise TypeError("Invalid input for output_mode")
+    check_bin_size(bin_size)
     models, _ = monotonic_models(fr, fr, cols, label_col, event_label, bin_method, bin_size)
 
     # one bin_assign per bin count: _apply_binning's `len(cuts[0]) + 1` label quirk assumes one bin_size per call

@@ -19,7 +19,7 @@ import numpy as np
 import pandas as pd
 
 from .. import engine, profile
-from ..data_transformer.transformers import compute_cutoffs, load_binning_model, save_binning_model
+from ..data_transformer.transformers import check_bin_size, compute_cutoffs, load_binning_model, save_binning_model
 from ..frame import as_frame
 from ..result import ResultFrame
 from .validations import check_distance_method, check_list_of_columns
@@ -94,6 +94,7 @@ def statistics(spark, idf_target, idf_source, list_of_cols="all", drop_cols=None
                model_directory="drift_statistics", print_impact=False):
     """Same signature as the reference (:18-41).  Returns [attribute, <metrics in PSI,HD,JSD,KS
     order>, flagged]; metrics are not rounded; flagged = 1 if any metric > threshold."""
+    check_bin_size(bin_size)
     tgt = as_frame(idf_target)
     src = as_frame(idf_source) if idf_source is not None else None
     if src is None and not pre_existing_source:

@@ -210,6 +210,10 @@ class BinModel:
         self.cutoffs = [list(map(float, c)) for c in cutoffs]
         self.exact = list(exact) if exact is not None else [None] * len(self.names)
         self.max_bins = max((len(c) + 1 for c in self.cutoffs), default=2)
+        if self.max_bins > _lib.MAX_BINS:
+            wide = [n for n, c in zip(self.names, self.cutoffs) if len(c) + 1 > _lib.MAX_BINS]
+            raise ValueError("binning model of %d bins (columns %s): at most %d bins per column are supported"
+                             % (self.max_bins, ", ".join(map(repr, wide)), _lib.MAX_BINS))
         specs = np.zeros(len(self.names), dtype=_SPEC_DT)
         raws, off = [], 0
         for i, (nme, cut) in enumerate(zip(self.names, self.cutoffs)):

@@ -36,6 +36,11 @@ extern "C" {
  * blocks of at most this many (every per-column result is independent of the other columns of the call). */
 #define ANV_MAX_LAUNCH_COLS 65535
 
+/* Most bins per column of the binning entry points (anv_hist, anv_moments_hist, anv_bin_assign): each CTA holds the
+ * column's whole threshold table in shared memory, 8 bytes per slot of the next power of two (131 KB at this limit).
+ * A wider model is refused with ANV_ERR_UNSUPPORTED. */
+#define ANV_MAX_BINS 16384
+
 typedef enum {
   ANV_OK = 0,
   ANV_ERR_INVALID = -1,   /* bad argument (null pointer, misaligned column, bad dtype ...) */
@@ -110,20 +115,21 @@ int anv_moments(const anv_column_t* cols, int n_cols, int64_t n_rows, anv_moment
  *      transformers.py:248-280, and the groupBy counts of drift_detector.py:252-264)
  * counts [dev] n_cols * count_stride uint64: slot 0 = nulls, slot b = rows in bin b.
  * The library zeroes `counts` on the stream before accumulating.
- * specs [dev] n_cols; cuts [dev] 8-byte threshold slots. count_stride >= max n_bins+1. */
+ * specs [dev] n_cols; cuts [dev] 8-byte threshold slots. count_stride >= max n_bins+1.
+ * n_bins <= ANV_MAX_BINS: count_stride > ANV_MAX_BINS + 1 is refused. */
 int anv_hist(const anv_column_t* cols, const anv_binspec_t* specs, const void* cuts, int n_cols,
              int64_t n_rows, uint64_t* counts, int count_stride, void* stream);
 
 /* ---- K1+K2 fused: moments AND histogram in ONE read of the frame (the target frame of
  *      drift_detector.statistics, whose cutoffs come from the source model,
- *      drift_detector.py:229-237). */
+ *      drift_detector.py:229-237).  Same count_stride limit as anv_hist: n_bins <= ANV_MAX_BINS. */
 int anv_moments_hist(const anv_column_t* cols, const anv_binspec_t* specs, const void* cuts, int n_cols,
                      int64_t n_rows, anv_moments_t* out, uint64_t* counts, int count_stride,
                      void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- bin-id materialisation (attribute_binning's returned frame, transformers.py:273-280)
  * out_bins [dev] int32: column c is written at out_bins + c * out_stride (elements,
- * out_stride >= n_rows and a multiple of 4); null rows get 0.  max_bins >= every n_bins. */
+ * out_stride >= n_rows and a multiple of 4); null rows get 0.  max_bins >= every n_bins, 2 <= max_bins <= ANV_MAX_BINS. */
 int anv_bin_assign(const anv_column_t* cols, const anv_binspec_t* specs, const void* cuts, int n_cols,
                    int64_t n_rows, int max_bins, int32_t* out_bins, int64_t out_stride, void* stream);
 

@@ -32,6 +32,18 @@ def test_column_block_limit_matches_header():
     assert int(re.search(r"#define ANV_MAX_LAUNCH_COLS (\d+)", h).group(1)) == _lib.MAX_LAUNCH_COLS == 65535
 
 
+def test_bin_limit_matches_header():
+    from anovos_b200 import _lib
+    h = open(os.path.join(ROOT, "include", "anovos_b200.h")).read()
+    assert int(re.search(r"#define ANV_MAX_BINS (\d+)", h).group(1)) == _lib.MAX_BINS == 16384
+    # every binning entry point checks against the constant, none against a literal of its own
+    src = open(os.path.join(ROOT, "anovos_b200", "csrc", "scan_host.cu")).read()
+    for fn in ("anv_hist", "anv_moments_hist", "anv_bin_assign"):
+        body = src[src.index('extern "C" int %s(' % fn):]
+        body = body[:body.index("\n}\n")]
+        assert "ANV_MAX_BINS" in body and not re.search(r"\b(4096|16384|16385)\b", body), fn
+
+
 def test_struct_layouts_match_header():
     from anovos_b200 import _lib, engine
     assert ctypes.sizeof(_lib.AnvColumn) == 24 and ctypes.sizeof(_lib.AnvMoments) == 64
