@@ -56,20 +56,9 @@ __device__ __forceinline__ void map_column(const int32_t* __restrict__ codes, co
       }
       store_quad<U>(dst, r, o);
     }
-    if constexpr (ENTRY_VALID) {
-      uint32_t word = keep << (4 * (lane & 7));
-      word |= __shfl_xor_sync(ANV_FULL, word, 1);
-      word |= __shfl_xor_sync(ANV_FULL, word, 2);
-      word |= __shfl_xor_sync(ANV_FULL, word, 4);
-      const int64_t w = r0 / 32 + (lane >> 3);
-      if ((lane & 7) == 0 && w * 32 < n_rows) sp.out_valid[w] = word;
-    }
+    if constexpr (ENTRY_VALID) store_quad_valid_bits(sp.out_valid, keep, r0, n_rows, lane);
   }
-  if constexpr (ENTRY_VALID) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) nulls += __shfl_down_sync(ANV_FULL, nulls, o);
-    if (lane == 0 && nulls) atomicAdd(n_null, nulls);
-  }
+  if constexpr (ENTRY_VALID) warp_add_count(n_null, nulls, lane);
 }
 
 template <typename U>

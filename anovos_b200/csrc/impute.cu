@@ -106,16 +106,9 @@ __device__ __forceinline__ void valid_not_nan_column(const T* __restrict__ src, 
       }
     }
     nan_count += __popc(nan);
-    uint32_t word = keep << (4 * (lane & 7));
-    word |= __shfl_xor_sync(ANV_FULL, word, 1);
-    word |= __shfl_xor_sync(ANV_FULL, word, 2);
-    word |= __shfl_xor_sync(ANV_FULL, word, 4);
-    const int64_t w = r0 / 32 + (lane >> 3);
-    if ((lane & 7) == 0 && w * 32 < n_rows) out[w] = word;
+    store_quad_valid_bits(out, keep, r0, n_rows, lane);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) nan_count += __shfl_down_sync(ANV_FULL, nan_count, o);
-  if (lane == 0 && nan_count) atomicAdd(n_nan, nan_count);
+  warp_add_count(n_nan, nan_count, lane);
 }
 
 __global__ void __launch_bounds__(ANV_BLOCK) valid_not_nan_kernel(const anv_column_t* __restrict__ cols, int64_t n_rows,

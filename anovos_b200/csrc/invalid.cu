@@ -118,14 +118,7 @@ __device__ __forceinline__ void flag_column(const anv_column_t& col, const anv_f
           if (idx[k] >= 0 && lane == __ffs(peers) - 1) atomicAdd(counts + idx[k], (unsigned long long)__popc(peers));
         }
       }
-      if (out_valid) {
-        uint32_t word = keep << (4 * (lane & 7));
-        word |= __shfl_xor_sync(ANV_FULL, word, 1);
-        word |= __shfl_xor_sync(ANV_FULL, word, 2);
-        word |= __shfl_xor_sync(ANV_FULL, word, 4);
-        const int64_t w = r0 / 32 + (lane >> 3);
-        if ((lane & 7) == 0 && w * 32 < n_rows) out_valid[w] = word;
-      }
+      if (out_valid) store_quad_valid_bits(out_valid, keep, r0, n_rows, lane);
     }
     if (SHARED && ++tiles == FLAG_FLUSH_TILES) {
       tiles = 0;

@@ -1,4 +1,5 @@
-// Four-rows-per-lane streaming helpers of the per-column transform passes (impute.cu, scale.cu).
+// Four-rows-per-lane streaming helpers of the per-column transform passes (impute.cu, scale.cu, encode.cu, transform.cu,
+// invalid.cu).
 //
 // A warp covers 128 consecutive rows per step, four per lane, so every lane moves its values with 128-bit loads and
 // stores (two for 8-byte types).  The validity word of 32 rows is loaded once, by one of the first four lanes, and
@@ -54,6 +55,24 @@ __device__ __forceinline__ uint32_t quad_valid_bits(const uint32_t* __restrict__
   uint32_t word = (lane < 4 && w < n_words) ? __ldg(validity + w) : 0u;
   word = __shfl_sync(ANV_FULL, word, lane >> 3);
   return (word >> (4 * (lane & 7))) & 0xFu;
+}
+
+// The inverse of quad_valid_bits: the 8 lanes of each 32-row word OR their 4 keep bits together and the word's first
+// lane stores it to the output bitmap.  Called by the whole warp (r0 is warp-uniform).
+__device__ __forceinline__ void store_quad_valid_bits(uint32_t* __restrict__ out, uint32_t keep, int64_t r0, int64_t n_rows, int lane) {
+  uint32_t word = keep << (4 * (lane & 7));
+  word |= __shfl_xor_sync(ANV_FULL, word, 1);
+  word |= __shfl_xor_sync(ANV_FULL, word, 2);
+  word |= __shfl_xor_sync(ANV_FULL, word, 4);
+  const int64_t w = r0 / 32 + (lane >> 3);
+  if ((lane & 7) == 0 && w * 32 < n_rows) out[w] = word;
+}
+
+// Adds the warp's sum of n to *counter with one atomic from lane 0, none when the sum is 0.  Called by the whole warp.
+__device__ __forceinline__ void warp_add_count(unsigned long long* __restrict__ counter, unsigned long long n, int lane) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n += __shfl_down_sync(ANV_FULL, n, o);
+  if (lane == 0 && n) atomicAdd(counter, n);
 }
 
 // Row tiles per column of a (row tiles, columns) grid: enough CTAs for ~16 per SM across the launch, never more than

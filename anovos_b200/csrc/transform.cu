@@ -279,18 +279,9 @@ __global__ void __launch_bounds__(ANV_BLOCK) transform_kernel(const anv_column_t
         default: store_as<int64_t>(dst, r, o); break;
       }
     }
-    if (nulls_out) {
-      uint32_t word = keep << (4 * (lane & 7));
-      word |= __shfl_xor_sync(ANV_FULL, word, 1);
-      word |= __shfl_xor_sync(ANV_FULL, word, 2);
-      word |= __shfl_xor_sync(ANV_FULL, word, 4);
-      const int64_t w = r0 / 32 + (lane >> 3);
-      if ((lane & 7) == 0 && w * 32 < n_rows) out_valid[w] = word;
-    }
+    if (nulls_out) store_quad_valid_bits(out_valid, keep, r0, n_rows, lane);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) nulls += __shfl_down_sync(ANV_FULL, nulls, o);
-  if (lane == 0 && nulls) atomicAdd(null_counts + c, nulls);
+  warp_add_count(null_counts + c, nulls, lane);
 }
 
 // ---- Box-Cox lambda search: the Kolmogorov-Smirnov statistics of every candidate from one sort ------------------------

@@ -21,15 +21,9 @@ from ..data_transformer.transformers import check_bin_size, compute_cutoffs
 from ..frame import as_frame
 from ..result import ResultFrame
 from ..shared.label_classes import label_bitmaps as _label_bitmaps, masked as _masked
-from ..shared.utils import attributeType_segregation
+from ..shared.utils import attributeType_segregation, names, unique
 
 _DEFAULT_ENC = {"bin_method": "equal_frequency", "bin_size": 10, "monotonicity_check": 0}
-
-
-def _names(x):
-    if isinstance(x, str):
-        return [s.strip() for s in x.split("|")]
-    return list(x)
 
 
 def _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_configs):
@@ -49,11 +43,7 @@ def _prepare(idf, list_of_cols, drop_cols, label_col, event_label, encoding_conf
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         num, cat, _ = attributeType_segregation(fr)
         list_of_cols = num + cat
-    drop = _names(drop_cols) + [label_col]
-    cols = []
-    for c in _names(list_of_cols):
-        if c not in drop and c not in cols:
-            cols.append(c)
+    cols = unique(names(list_of_cols), names(drop_cols) + [label_col])
     if any(c not in fr.columns for c in cols) or not cols:
         raise TypeError("Invalid input for Column(s)")
     ev_w, nev_w, n_event = _label_bitmaps(fr, label_col, event_label)

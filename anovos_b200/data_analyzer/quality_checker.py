@@ -25,14 +25,8 @@ import pandas as pd
 from .. import _lib, engine, profile
 from ..frame import Column, ColumnFrame, as_frame, pack_bits_device
 from ..result import ResultFrame
-from ..shared.utils import attributeType_segregation, jvm_double_str, spark_round
+from ..shared.utils import attributeType_segregation, jvm_double_str, names, spark_round, unique
 from .stats_generator import _mode_str, measures_of_cardinality, missingCount_computation
-
-
-def _names(x):
-    if isinstance(x, str):
-        return [s.strip() for s in x.split("|")]
-    return list(x)
 
 
 def _as_bool(v, what):
@@ -41,11 +35,6 @@ def _as_bool(v, what):
     if str(v).lower() == "false":
         return False
     raise TypeError("Non-Boolean input for " + what)
-
-
-def _unique(cols, drop):
-    drop = set(drop)
-    return [c for c in dict.fromkeys(cols) if c not in drop]     # first-seen order; sets keep wide frames linear
 
 
 def _read_stats(spec, columns):
@@ -67,7 +56,7 @@ def _row_cols(fr, list_of_cols, drop_cols):
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         num, cat, _ = attributeType_segregation(fr)
         list_of_cols = num + cat
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     known = set(fr.columns)
     if any(c not in known for c in cols) or len(cols) == 0:
         raise TypeError("Invalid input for Column(s)")
@@ -198,7 +187,7 @@ def nullColumns_detection(spark, idf, list_of_cols="missing", drop_cols=[], trea
         list_of_cols = num + cat
     if isinstance(list_of_cols, str) and list_of_cols == "missing":
         list_of_cols = missing_cols
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     if not cols:
         warnings.warn("No Null Detection - No column(s) to analyze")
         return fr, ResultFrame(pd.DataFrame(columns=["attribute", "missing_count", "missing_pct"]))
@@ -257,7 +246,7 @@ def _discrete(fr, list_of_cols, drop_cols):
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         num, cat, _ = attributeType_segregation(fr)
         list_of_cols = num + cat
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(c not in fr.columns for c in cols):
         raise TypeError("Invalid input for Column(s)")
     types = dict(fr.dtypes)
@@ -473,7 +462,7 @@ def outlier_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_si
             return fr
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = num_cols
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     empty_print = ResultFrame(pd.DataFrame(columns=_PRINT_COLS[:3]))
     if not cols:
         warnings.warn("No Outlier Check - No numerical column to analyze")
@@ -546,7 +535,7 @@ def outlier_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_si
                 raise NotImplementedError("outlier treatment of a row-partitioned frame is not implemented "
                                           "(detection with print_impact=True is)")
             hist = engine.histogram(fr, model)
-        new_cols = OrderedDict((n, fr.column(n)) for n in fr.columns)
+        made = OrderedDict()
         keep = torch.ones(fr.n_rows, dtype=torch.bool, device=ids.device) if need_rows else None
         for i, c in enumerate(cols):
             flags_of_bin = specs[i][1]
@@ -584,20 +573,20 @@ def outlier_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_si
                     out = torch.where(flag == -1, torch.tensor(float(lo), dtype=torch.float64, device=out.device), out)
                 if hi is not None:
                     out = torch.where(flag == 1, torch.tensor(float(hi), dtype=torch.float64, device=out.device), out)
-                new_cols[name] = Column(name, "double", fr.n_rows, dev=out, dev_valid=v, anv_dtype=_lib.ANV_F64,
-                                        null_count=src.null_count)
+                made[name] = Column(name, "double", fr.n_rows, dev=out, dev_valid=v, anv_dtype=_lib.ANV_F64,
+                                    null_count=src.null_count)
             elif treatment_method == "null_replacement":
                 valid = (ids[i] != 0) & (flag == 0)
                 nv = None if bool(valid.all()) else pack_bits_device(valid)
-                new_cols[name] = Column(name, src.sdtype, fr.n_rows, dev=d, dev_valid=nv, anv_dtype=src.anv_dtype,
-                                        dictionary=src.dictionary)
+                made[name] = Column(name, src.sdtype, fr.n_rows, dev=d, dev_valid=nv, anv_dtype=src.anv_dtype,
+                                    dictionary=src.dictionary)
             else:
                 keep &= flag == 0
         if need_rows:
             if treatment_method == "row_removal":
                 odf = fr.filter_rows(keep)
             else:
-                odf = ColumnFrame(new_cols, fr.n_rows)
+                odf = fr.with_columns(made)
     rows += [(c, 0, 0, 1) for c in (skewed if print_impact else [])]
     if treatment and output_mode == "replace":
         odf = odf.select(column_order)
@@ -664,7 +653,7 @@ def _with_flags_nulled(fr, cols, bitmaps, counts, output_mode, append_cols, sche
     data under a new bitmap.  replace: the column moves to the end of the frame (the reference drops it and re-adds it);
     append: <c>_invalid is appended for the columns in `append_cols`.  schema=True: names, dtypes and dictionaries only
     (the schema of a row-partitioned result)."""
-    new = OrderedDict((n, fr.column(n)) for n in fr.columns)
+    made = OrderedDict()
     for c, bm, cnt in zip(cols, bitmaps, counts):
         if output_mode == "append" and c not in append_cols:
             continue
@@ -679,11 +668,9 @@ def _with_flags_nulled(fr, cols, bitmaps, counts, output_mode, append_cols, sche
             d, v = src.device()
             nulls = None if base is None else base + int(np.sum(cnt))
         name = c if output_mode == "replace" else c + "_invalid"
-        if output_mode == "replace":
-            del new[c]
-        new[name] = Column(name, src.sdtype, fr.n_rows, dev=d, dev_valid=bm if bm is not None else v,
-                           anv_dtype=src.anv_dtype, null_count=nulls, dictionary=src.dictionary)
-    return ColumnFrame(new, fr.n_rows)
+        made[name] = Column(name, src.sdtype, fr.n_rows, dev=d, dev_valid=bm if bm is not None else v,
+                            anv_dtype=src.anv_dtype, null_count=nulls, dictionary=src.dictionary)
+    return fr.with_columns(made, drop=list(made) if output_mode == "replace" else ())
 
 
 def invalidEntries_detection(spark, idf, list_of_cols="all", drop_cols=[], detection_type="auto", invalid_entries=[],
@@ -706,7 +693,7 @@ def invalidEntries_detection(spark, idf, list_of_cols="all", drop_cols=[], detec
     fr = as_frame(idf)
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = [n for n, t in fr.dtypes if t in ("string", "int", "bigint", "long")]
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(c not in fr.columns for c in cols):
         raise TypeError("Invalid input for Column(s)")
     if not cols:

@@ -16,25 +16,9 @@ import pandas as pd
 from .. import profile
 from ..frame import as_frame
 from ..result import ResultFrame
-from ..shared.utils import attributeType_segregation, jvm_double_str, spark_round, spark_round_array
+from ..shared.utils import attributeType_segregation, jvm_double_str, names, spark_round, spark_round_array, unique
 
 _R = spark_round
-
-
-def _names(x):
-    if isinstance(x, str):
-        return [s.strip() for s in x.split("|")]
-    return list(x)
-
-
-def _unique(cols, drop):
-    # the reference does list(set(...)) - arbitrary order; we keep first-seen order (SURVEY C#7)
-    seen, out = set(), []
-    for c in cols:
-        if c not in drop and c not in seen:
-            seen.add(c)
-            out.append(c)
-    return out
 
 
 def _empty(cols):
@@ -117,7 +101,7 @@ def global_summary(spark, idf, list_of_cols="all", drop_cols=[], print_impact=Fa
     fr = as_frame(idf)
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = fr.columns
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(c not in fr.columns for c in cols) or not cols:
         raise TypeError("Invalid input for Column(s)")
     num, cat, other = attributeType_segregation(fr.select(cols))
@@ -145,7 +129,7 @@ def _discrete_cols(fr, list_of_cols, drop_cols, allow_empty=False):
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         num, cat, _ = attributeType_segregation(fr)
         list_of_cols = num + cat
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(c not in fr for c in cols) or (not cols and not allow_empty):
         raise TypeError("Invalid input for Column(s)")
     bad = [c for c in cols if fr.column(c).kind == "other"]
@@ -159,7 +143,7 @@ def _numeric_cols(fr, list_of_cols, drop_cols):
     num = attributeType_segregation(fr)[0]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = num
-    cols = _unique(_names(list_of_cols), _names(drop_cols))
+    cols = unique(names(list_of_cols), names(drop_cols))
     numset = set(num)
     if any(c not in numset for c in cols):
         raise TypeError("Invalid input for Column(s)")

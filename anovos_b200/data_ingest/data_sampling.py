@@ -19,6 +19,7 @@ import numpy as np
 
 from .. import _lib, profile
 from ..frame import ColumnFrame, as_frame
+from ..shared.utils import names, unique
 
 
 def fraction_threshold(fraction: float) -> int:
@@ -26,10 +27,6 @@ def fraction_threshold(fraction: float) -> int:
     f = Fraction(float(fraction)) * (1 << 53)
     k = -((-f.numerator) // f.denominator)
     return int(min(max(k, 0), 1 << 53))
-
-
-def _names(x):
-    return [s.strip() for s in x.split("|")] if isinstance(x, str) else list(x)
 
 
 def _require(ok, message):
@@ -125,8 +122,7 @@ def _checked_strata(fr, strata_cols, drop_cols, stratified_type, unique_threshol
     _require(stratified_type in ("population", "balanced"), "Invalid input for stratified_type")
     if isinstance(strata_cols, str) and strata_cols == "all":
         strata_cols = fr.columns
-    strata_cols, drop_cols = _names(strata_cols), _names(drop_cols)
-    strata_cols = list(dict.fromkeys(e for e in strata_cols if e not in drop_cols))
+    strata_cols = unique(names(strata_cols), names(drop_cols))
     _require(strata_cols, "Missing strata_cols value")
     for col in strata_cols:
         _require(col in fr.columns, "Invalid input for strata_cols: " + col + " does not exist")

@@ -22,13 +22,7 @@ import numpy as np
 
 from .. import _lib, engine, profile
 from ..frame import Column, ColumnFrame, as_frame
-from ..shared.utils import attributeType_segregation
-
-
-def _names(x):
-    if isinstance(x, str):
-        return [s.strip() for s in x.split("|")]
-    return list(x)
+from ..shared.utils import attributeType_segregation, names, unique
 
 
 def _model_dir(model_path):
@@ -94,31 +88,53 @@ def _labels(cut, n_over_cut):
     return out
 
 
+def _per_chunk(fr, fn):
+    """fn(frame) -> frame, lazily on each chunk of a row-partitioned frame (whose schema is fn of its schema frame)."""
+    if getattr(fr, "is_partitioned", False):
+        return fr.map_chunks(fn(fr._schema), fn)
+    return fn(fr)
+
+
+def _out_column(fr, src, name, anv_dtype, data, valid=None, null_count=0, sdtype=None, dictionary=None):
+    """Output column `name` of a pass over column `src` of fr: with the bitmap and null count the pass made, or, where it
+    made no bitmap (valid None), with the source's."""
+    if valid is None:
+        s = fr.column(src)
+        valid, null_count = s.device()[1], s.null_count
+    else:
+        null_count = int(null_count)
+    return Column(name, sdtype or _SDTYPE_OF_ANV[anv_dtype], fr.n_rows, dev=data, dev_valid=valid, anv_dtype=anv_dtype,
+                  null_count=null_count, dictionary=dictionary)
+
+
+def _null_column(fr, src, name, anv_dtype):
+    """An all-null output column `name` on the device of column `src`."""
+    torch = _lib.require_cuda()
+    dev = fr.column(src).device()[0].device
+    return Column(name, _SDTYPE_OF_ANV[anv_dtype], fr.n_rows,
+                  dev=torch.zeros(max(fr.n_rows, 1), dtype=getattr(torch, engine._TORCH_OF_ANV[anv_dtype]), device=dev)[:fr.n_rows],
+                  dev_valid=torch.zeros(max((fr.n_rows + 31) // 32, 1), dtype=torch.int32, device=dev),
+                  anv_dtype=anv_dtype, null_count=fr.n_rows)
+
+
 def _apply_binning(fr: ColumnFrame, cols, cuts, lohi, bin_dtype, output_mode) -> ColumnFrame:
     """bucket_label (:248-280) for every value of `cols` with the given cutoffs -> new frame."""
     bm = engine.BinModel(fr, cols, cuts, lohi)
     ids = engine.bin_assign(fr, bm)                         # [n_cols, n_rows] int32, 0 = null
     n_over = len(cuts[0]) + 1                               # `len(bin_cutoffs[0]) + 1` quirk (:269)
-    new_cols = OrderedDict((n, fr.column(n)) for n in fr.columns)
+    made = OrderedDict()
     for i, c in enumerate(cols):
-        src = fr.column(c)
-        _, v = src.device()
         data = ids[i]
         if len(cuts[i]) + 1 != n_over:                      # only reachable with a hand-made model
             data = data.clone()
             data[data == len(cuts[i]) + 1] = n_over
+        name = c if output_mode == "replace" else c + "_binned"
         if bin_dtype == "numerical":
-            col = Column(c, "int", fr.n_rows, dev=data, dev_valid=v, anv_dtype=_lib.ANV_I32,
-                         null_count=src.null_count)
+            made[name] = _out_column(fr, c, name, _lib.ANV_I32, data)
         else:
-            col = Column(c, "string", fr.n_rows, dev=(data - 1).clamp_(min=0), dev_valid=v, anv_dtype=_lib.ANV_I32,
-                         null_count=src.null_count, dictionary=_labels(cuts[i], len(cuts[0])))
-        if output_mode == "replace":
-            new_cols[c] = col
-        else:
-            col.name = c + "_binned"
-            new_cols[c + "_binned"] = col
-    return ColumnFrame(new_cols, fr.n_rows)
+            made[name] = _out_column(fr, c, name, _lib.ANV_I32, (data - 1).clamp_(min=0), sdtype="string",
+                                     dictionary=_labels(cuts[i], len(cuts[0])))
+    return fr.with_columns(made)
 
 
 def attribute_binning(spark, idf, list_of_cols="all", drop_cols=[], method_type="equal_range", bin_size=10,
@@ -130,11 +146,7 @@ def attribute_binning(spark, idf, list_of_cols="all", drop_cols=[], method_type=
     num_cols = attributeType_segregation(fr)[0]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = num_cols
-    drop = _names(drop_cols)
-    cols = []
-    for c in _names(list_of_cols):
-        if c not in drop and c not in cols:
-            cols.append(c)
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(c not in num_cols for c in cols):
         raise TypeError("Invalid input for Column(s)")
     if not cols:
@@ -163,12 +175,8 @@ def attribute_binning(spark, idf, list_of_cols="all", drop_cols=[], method_type=
     if not cols:
         return fr
 
-    if getattr(fr, "is_partitioned", False):
-        # lazy per-chunk transform with the (global) model: the binned frame is partitioned like its input
-        schema = _apply_binning(fr._schema, cols, cuts, lohi, bin_dtype, output_mode)
-        odf = fr.map_chunks(schema, lambda ch: _apply_binning(ch, cols, cuts, lohi, bin_dtype, output_mode))
-    else:
-        odf = _apply_binning(fr, cols, cuts, lohi, bin_dtype, output_mode)
+    # a partitioned frame is binned lazily per chunk with the (global) model: the result is partitioned like its input
+    odf = _per_chunk(fr, lambda f: _apply_binning(f, cols, cuts, lohi, bin_dtype, output_mode))
     if print_impact:
         from ..data_analyzer.stats_generator import uniqueCount_computation
         out_cols = cols if output_mode == "replace" else [c + "_binned" for c in cols]
@@ -208,11 +216,7 @@ def monotonic_binning(spark, idf, list_of_cols="all", drop_cols=[], label_col="l
     num_cols = attributeType_segregation(fr)[0]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = num_cols
-    drop = _names(drop_cols) + [label_col]
-    cols = []
-    for c in _names(list_of_cols):
-        if c not in drop and c not in cols:
-            cols.append(c)
+    cols = unique(names(list_of_cols), names(drop_cols) + [label_col])
     if any(c not in num_cols for c in cols):
         raise TypeError("Invalid input for Column(s)")
     if not cols:
@@ -232,12 +236,7 @@ def monotonic_binning(spark, idf, list_of_cols="all", drop_cols=[], label_col="l
         grp = [c for c in cols if models[c][0] == n]
         cuts = [models[c][1] for c in grp]
         lohi = [models[c][2] for c in grp]
-        if getattr(odf, "is_partitioned", False):
-            schema = _apply_binning(odf._schema, grp, cuts, lohi, bin_dtype, output_mode)
-            odf = odf.map_chunks(schema, lambda ch, g=grp, cu=cuts, lh=lohi: _apply_binning(ch, g, cu, lh, bin_dtype,
-                                                                                              output_mode))
-        else:
-            odf = _apply_binning(odf, grp, cuts, lohi, bin_dtype, output_mode)
+        odf = _per_chunk(odf, lambda f, g=grp, cu=cuts, lh=lohi: _apply_binning(f, g, cu, lh, bin_dtype, output_mode))
     if output_mode == "append":
         order = list(fr.columns) + [c + "_binned" for c in cols]
         if list(odf.columns) != order:
@@ -356,12 +355,11 @@ def _nan_view(fr, cols):
     if getattr(fr, "is_partitioned", False):
         return fr.map_chunks(fr._schema, lambda ch: _nan_view(ch, cols))
     words, _ = engine.valid_not_nan(fr, cols)
-    new = OrderedDict((n, fr.column(n)) for n in fr.columns)
+    made = OrderedDict()
     for i, c in enumerate(cols):
         src = fr.column(c)
-        d, _v = src.device()
-        new[c] = Column(c, src.sdtype, fr.n_rows, dev=d, dev_valid=words[i], anv_dtype=src.anv_dtype)
-    return ColumnFrame(new, fr.n_rows)
+        made[c] = Column(c, src.sdtype, fr.n_rows, dev=src.device()[0], dev_valid=words[i], anv_dtype=src.anv_dtype)
+    return fr.with_columns(made)
 
 
 def _surrogates(fr, cols, method_type):
@@ -420,9 +418,10 @@ def _fill_dictionary(col, value):
         return list(dic) + [value], len(dic)
 
 
-def _apply_plan(fr, plan: _Plan, order):
-    """Run the recasts and fills of `plan` on a (resident) frame in ONE anv_impute_fill launch; `order` = the output
-    column names, in order."""
+def _apply_plan(fr, plan: _Plan, replaced):
+    """Run the recasts and fills of `plan` on a (resident) frame in ONE anv_impute_fill launch.  The recasts stay in
+    place; the fills, in plan order, replace a column of their name in place or follow the columns after `replaced` is
+    dropped."""
     srcs, outs_dt, flags, bits = [], [], [], []
     for c in plan.recast:
         srcs.append(c)
@@ -435,19 +434,16 @@ def _apply_plan(fr, plan: _Plan, order):
         flags.append(fl)
         bits.append(0 if val is None else engine.fill_bits(val, od))
     data = engine.impute_fill(fr, srcs, outs_dt, flags, bits)
-    made = {}
+    made = OrderedDict()
     for c, d in zip(plan.recast, data[:len(plan.recast)]):
-        s = fr.column(c)
-        _, v = s.device()
-        made[c] = Column(c, "double", fr.n_rows, dev=d, dev_valid=v, anv_dtype=_lib.ANV_F64, null_count=s.null_count)
+        made[c] = _out_column(fr, c, c, _lib.ANV_F64, d)
     for (name, src, od, fl, val, dic), d in zip(plan.fills, data[len(plan.recast):]):
-        s = fr.column(src)
-        v, nc = None, 0
+        sd = "string" if dic is not None else None
         if val is None:                                    # a null fill leaves the nulls where they are
-            v, nc = s.device()[1], s.null_count
-        sd = "string" if dic is not None else _SDTYPE_OF_ANV[od]
-        made[name] = Column(name, sd, fr.n_rows, dev=d, dev_valid=v, anv_dtype=od, null_count=nc, dictionary=dic)
-    return ColumnFrame(OrderedDict((n, made[n] if n in made else fr.column(n)) for n in order), fr.n_rows)
+            made[name] = _out_column(fr, src, name, od, d, sdtype=sd, dictionary=dic)
+        else:
+            made[name] = Column(name, sd or _SDTYPE_OF_ANV[od], fr.n_rows, dev=d, anv_dtype=od, null_count=0, dictionary=dic)
+    return fr.with_columns(made, drop=replaced)
 
 
 def _impact(spark, odf, missing_df, list_of_cols, num_cols, cat_cols, missing_cols, output_mode):
@@ -492,8 +488,7 @@ def imputation_MMM(spark, idf, list_of_cols="missing", drop_cols=[], method_type
         list_of_cols = num_all + cat_all
     if isinstance(list_of_cols, str) and list_of_cols == "missing":
         list_of_cols = [x for x in missing_cols if x in num_all + cat_all]
-    drop = _names(drop_cols)
-    list_of_cols = [c for c in dict.fromkeys(_names(list_of_cols)) if c not in drop]
+    list_of_cols = unique(names(list_of_cols), names(drop_cols))
     if not list_of_cols:
         warnings.warn("No Imputation performed- No column(s) to impute")
         return fr
@@ -580,26 +575,22 @@ def imputation_MMM(spark, idf, list_of_cols="missing", drop_cols=[], method_type
             save_cat_imputer(model_path, cat_cols, params)
 
     # :1638-1642 - only columns with nulls keep their `_imputed`; "replace" moves it into the original's name, at the end
-    order = [c for c in fr.columns]
+    replaced = []
     kept = list(created)
     for i in num_cols + cat_cols:
         if i not in missing_cols:
             kept = [k for k in kept if k != i + "_imputed"]
         elif output_mode == "replace":
-            order = [c for c in order if c != i]
+            replaced.append(i)
     renamed = {}
     for k in kept:
         base = k[:-8] if k.endswith("_imputed") else None
         if output_mode == "replace" and base in missing_cols and base in num_cols + cat_cols:
             renamed[k] = base
-    order = order + [renamed.get(k, k) for k in kept]
-    plan.recast = [c for c in recast if c in order]
+    plan.recast = [c for c in recast if c not in replaced]       # a replaced column's output is its fill, not its recast
     plan.fills = [(renamed.get(f[0], f[0]),) + f[1:] for f in plan.fills if f[0] in kept]
 
-    if getattr(fr, "is_partitioned", False):
-        odf = fr.map_chunks(_apply_plan(fr._schema, plan, order), lambda ch: _apply_plan(ch, plan, order))
-    else:
-        odf = _apply_plan(fr, plan, order)
+    odf = _per_chunk(fr, lambda f: _apply_plan(f, plan, replaced))
     if print_impact:
         _impact(spark, odf, missing_df, list_of_cols, num_cols, cat_cols, missing_cols, output_mode).show(len(list_of_cols), False)
     return odf
@@ -621,8 +612,7 @@ def _scale_cols(fr, list_of_cols, drop_cols, output_mode, what):
     num_cols = attributeType_segregation(fr)[0]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = num_cols
-    drop = _names(drop_cols)
-    cols = [c for c in dict.fromkeys(_names(list_of_cols)) if c not in drop]
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(c not in num_cols for c in cols):
         raise TypeError("Invalid input for Column(s)")
     if not cols:
@@ -774,40 +764,13 @@ def _apply_scaling(fr, cols, specs, output_mode):
     name and position; "append": `<c>_scaled` after all existing columns, in list order."""
     run = [i for i, s in enumerate(specs) if s is not None]
     data, valid, nulls = engine.scale_columns(fr, [cols[i] for i in run], [specs[i] for i in run])
-    made = {}
-    for k, i in enumerate(run):
-        src = fr.column(cols[i])
-        od = specs[i][1]
-        if specs[i][2] & _lib.SCALE_NAN_TO_NULL:
-            v, nc = valid[k], int(nulls[k])
-        else:
-            v, nc = src.device()[1], src.null_count
-        made[cols[i]] = Column(cols[i], _SDTYPE_OF_ANV[od], fr.n_rows, dev=data[k], dev_valid=v, anv_dtype=od, null_count=nc)
-    for i, s in enumerate(specs):
-        if s is None:
-            d, _ = fr.column(cols[i]).device()
-            torch = _lib.require_cuda()
-            made[cols[i]] = Column(cols[i], "double", fr.n_rows, dev=torch.zeros(max(fr.n_rows, 1), dtype=torch.float64,
-                                                                                  device=d.device)[:fr.n_rows],
-                                   dev_valid=torch.zeros(max((fr.n_rows + 31) // 32, 1), dtype=torch.int32, device=d.device),
-                                   anv_dtype=_lib.ANV_F64, null_count=fr.n_rows)
-    new = OrderedDict()
-    for n in fr.columns:
-        new[n] = made[n] if output_mode == "replace" and n in made else fr.column(n)
-    if output_mode == "append":
-        for c in cols:
-            if c in made:
-                col = made[c]
-                col.name = c + "_scaled"
-                new[col.name] = col
-    return ColumnFrame(new, fr.n_rows)
-
-
-def _scaled_frame(fr, cols, specs, output_mode):
-    if getattr(fr, "is_partitioned", False):
-        schema = _apply_scaling(fr._schema, cols, specs, output_mode)
-        return fr.map_chunks(schema, lambda ch: _apply_scaling(ch, cols, specs, output_mode))
-    return _apply_scaling(fr, cols, specs, output_mode)
+    out = dict(zip(run, zip(data, valid, nulls)))
+    made = OrderedDict()
+    for i, c in enumerate(cols):
+        name = c if output_mode == "replace" else c + "_scaled"
+        made[name] = _null_column(fr, c, name, _lib.ANV_F64) if specs[i] is None else \
+            _out_column(fr, c, name, specs[i][1], *out[i])
+    return fr.with_columns(made)
 
 
 def _describe_value(v, sdtype):
@@ -871,7 +834,7 @@ def z_standardization(spark, idf, list_of_cols="all", drop_cols=[], pre_existing
                       + str(excluded))
     kept = [c for c in cols if c not in excluded]
     specs = [_div_spec(p[0], p[1]) for c, p in zip(cols, params) if c not in excluded]
-    odf = _scaled_frame(fr, kept, specs, output_mode)
+    odf = _per_chunk(fr, lambda f: _apply_scaling(f, kept, specs, output_mode))
     if not pre_existing_model and model_path != "NA":
         _save_param_model(model_path, "z", cols, params)
     if print_impact:
@@ -895,7 +858,7 @@ def IQR_standardization(spark, idf, list_of_cols="all", drop_cols=[], pre_existi
     kept = [c for c in cols if c not in excluded]
     specs = [_div_spec(p[1], None if p[2] is None or p[0] is None else p[2] - p[0])
              for c, p in zip(cols, params) if c not in excluded]
-    odf = _scaled_frame(fr, kept, specs, output_mode)
+    odf = _per_chunk(fr, lambda f: _apply_scaling(f, kept, specs, output_mode))
     if not pre_existing_model and model_path != "NA":
         _save_param_model(model_path, "iqr", cols, params)
     if print_impact:
@@ -922,7 +885,8 @@ def normalization(idf, list_of_cols="all", drop_cols=[], pre_existing_model=Fals
         maxs = [float(mom[c]["max"]) if int(mom[c]["n_valid"]) else -_DOUBLE_MAX for c in cols]
         if model_path != "NA":
             save_minmax_model(model_path, lo, hi, mins, maxs)
-    odf = _scaled_frame(fr, cols, [minmax_spec(a, b, lo, hi) for a, b in zip(mins, maxs)], output_mode)
+    specs = [minmax_spec(a, b, lo, hi) for a, b in zip(mins, maxs)]
+    odf = _per_chunk(fr, lambda f: _apply_scaling(f, cols, specs, output_mode))
     if print_impact:
         _print_impact(fr, odf, cols, cols if output_mode == "replace" else [c + "_scaled" for c in cols])
     return odf
@@ -1000,8 +964,7 @@ def _transform_cols(fr, list_of_cols, drop_cols):
     num_cols = attributeType_segregation(fr)[0]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = num_cols
-    drop = _names(drop_cols)
-    cols = [c for c in dict.fromkeys(_names(list_of_cols)) if c not in drop]
+    cols = unique(names(list_of_cols), names(drop_cols))
     if len(cols) == 0 or any(c not in num_cols for c in cols):
         raise TypeError("Invalid input for Column(s)")
     sdt = dict(fr.dtypes)
@@ -1014,44 +977,13 @@ def _transform_cols(fr, list_of_cols, drop_cols):
 def _apply_transform(fr, cols, specs, out_names):
     """Write op(col) for each (col, spec) under its output name -> new frame: a name that exists keeps its position (the
     reference's withColumn), a new one goes after all existing columns, in list order."""
-    torch = None
     run = [i for i, s in enumerate(specs) if s[0] is not None]
     data, valid, nulls = engine.transform_columns(fr, [cols[i] for i in run], [specs[i] for i in run])
-    made = {}
-    for k, i in enumerate(run):
-        src = fr.column(cols[i])
-        od = specs[i][1]
-        if valid[k] is not None:
-            v, nc = valid[k], int(nulls[k])
-        else:
-            v, nc = src.device()[1], src.null_count
-        made[out_names[i]] = Column(out_names[i], _SDTYPE_OF_ANV[od], fr.n_rows, dev=data[k], dev_valid=v, anv_dtype=od,
-                                    null_count=nc)
-    for i, s in enumerate(specs):
-        if s[0] is None:
-            torch = torch or _lib.require_cuda()
-            d, _ = fr.column(cols[i]).device()
-            od = s[1]
-            made[out_names[i]] = Column(out_names[i], _SDTYPE_OF_ANV[od], fr.n_rows,
-                                        dev=torch.zeros(max(fr.n_rows, 1), dtype=getattr(torch, engine._TORCH_OF_ANV[od]),
-                                                        device=d.device)[:fr.n_rows],
-                                        dev_valid=torch.zeros(max((fr.n_rows + 31) // 32, 1), dtype=torch.int32,
-                                                              device=d.device),
-                                        anv_dtype=od, null_count=fr.n_rows)
-    new = OrderedDict()
-    for n in fr.columns:
-        new[n] = made.pop(n) if n in made else fr.column(n)
-    for n in out_names:
-        if n in made:
-            new[n] = made.pop(n)
-    return ColumnFrame(new, fr.n_rows)
-
-
-def _transformed_frame(fr, cols, specs, out_names):
-    if getattr(fr, "is_partitioned", False):
-        schema = _apply_transform(fr._schema, cols, specs, out_names)
-        return fr.map_chunks(schema, lambda ch: _apply_transform(ch, cols, specs, out_names))
-    return _apply_transform(fr, cols, specs, out_names)
+    out = dict(zip(run, zip(data, valid, nulls)))
+    made = OrderedDict()
+    for i, (c, name, s) in enumerate(zip(cols, out_names, specs)):
+        made[name] = _null_column(fr, c, name, s[1]) if s[0] is None else _out_column(fr, c, name, s[1], *out[i])
+    return fr.with_columns(made)
 
 
 def feature_transformation(idf, list_of_cols="all", drop_cols=[], method_type="sqrt", N=None, output_mode="replace",
@@ -1070,7 +1002,7 @@ def feature_transformation(idf, list_of_cols="all", drop_cols=[], method_type="s
         out_names = [c + "_" + method_type[:-1] + str(N) for c in cols]
     else:
         out_names = [c + "_" + method_type for c in cols]
-    odf = _transformed_frame(fr, cols, specs, out_names)
+    odf = _per_chunk(fr, lambda f: _apply_transform(f, cols, specs, out_names))
     if print_impact:
         print("Before:")
         describe(fr, cols).show(5, False)
@@ -1167,7 +1099,7 @@ def boxcox_transformation(idf, list_of_cols="all", drop_cols=[], boxcox_lambda=N
         return idf
     specs = [(_lib.TF_LN, _lib.ANV_F64, 0, 0.0) if lam == 0 else (_lib.TF_POW, _lib.ANV_F64, 0, float(lam)) for _, lam in run]
     out_names = [c + "_bxcx_" + str(lam) if output_mode == "append" else c for c, lam in run]
-    odf = _transformed_frame(fr, [c for c, _ in run], specs, out_names)
+    odf = _per_chunk(fr, lambda f: _apply_transform(f, [c for c, _ in run], specs, out_names))
     if print_impact:
         print("Transformed Columns: ", cols)
         print("Best BoxCox Parameter(s): ", lambdas)
@@ -1196,10 +1128,6 @@ _PRINT_TYPE = {"string": "string", "int": "integer", "bigint": "long", "long": "
 
 def _utf8(s):
     return s.encode("utf-8")
-
-
-def _split(x):
-    return [s.strip() for s in x.split("|")] if isinstance(x, str) else list(x)
 
 
 def _present(fr, cols):
@@ -1308,14 +1236,9 @@ def _apply_label(fr, cols, labels, output_mode):
     data, _, _ = engine.code_map(fr, cols, tables, [None] * len(cols))
     made = OrderedDict()
     for c, d in zip(cols, data):
-        src = fr.column(c)
         name = c if output_mode == "replace" else c + "_index"
-        made[name] = Column(name, "int", fr.n_rows, dev=d, dev_valid=src.device()[1], anv_dtype=_lib.ANV_I32,
-                            null_count=src.null_count)
-    new = OrderedDict((n, made[n] if n in made else fr.column(n)) for n in fr.columns)
-    for n, col in made.items():
-        new.setdefault(n, col)
-    return ColumnFrame(new, fr.n_rows)
+        made[name] = _out_column(fr, c, name, _lib.ANV_I32, d)
+    return fr.with_columns(made)
 
 
 def _apply_onehot(fr, cols, labels, output_mode):
@@ -1330,18 +1253,12 @@ def _apply_onehot(fr, cols, labels, output_mode):
                                 % (c, len(labels[c]) + 1, need / 1e9, free / 1e9))
     idx = [_label_index(fr.column(c).dictionary, labels[c]) for c in cols]
     outs = engine.one_hot(fr, cols, idx, [len(labels[c]) + 1 for c in cols])
-    new = OrderedDict((n, fr.column(n)) for n in fr.columns if not (output_mode == "replace" and n in cols))
+    made = OrderedDict()
     for c, o in zip(cols, outs):
         for j in range(len(labels[c]) + 1):
             name = "%s_%d" % (c, j)
-            new[name] = Column(name, "int", fr.n_rows, dev=o[j], anv_dtype=_lib.ANV_I32, null_count=0)
-    return ColumnFrame(new, fr.n_rows)
-
-
-def _per_chunk(fr, fn):
-    if getattr(fr, "is_partitioned", False):
-        return fr.map_chunks(fn(fr._schema), fn)
-    return fn(fr)
+            made[name] = Column(name, "int", fr.n_rows, dev=o[j], anv_dtype=_lib.ANV_I32, null_count=0)
+    return fr.with_columns(made, drop=cols if output_mode == "replace" else ())
 
 
 def _summary_value(v, sdtype):
@@ -1398,7 +1315,7 @@ def cat_to_num_unsupervised(spark, idf, list_of_cols="all", drop_cols=[], method
     cat_cols = attributeType_segregation(fr)[1]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = cat_cols
-    list_of_cols, drop_cols = _split(list_of_cols), _split(drop_cols)
+    list_of_cols, drop_cols = names(list_of_cols), names(drop_cols)
     if any(x not in cat_cols for x in list_of_cols):
         raise TypeError("Invalid input for Column(s)")
     if method_type not in ("onehot_encoding", "label_encoding"):
@@ -1412,7 +1329,7 @@ def cat_to_num_unsupervised(spark, idf, list_of_cols="all", drop_cols=[], method
     skip = [c for c in wanted if c in over and c not in drop_cols]
     if skip:
         warnings.warn("Columns dropped from encoding due to high cardinality: " + ",".join(skip))
-    cols = [c for c in wanted if c not in drop_cols + skip]
+    cols = unique(wanted, drop_cols + skip)
     if not cols:
         warnings.warn("No Encoding Computation - No categorical column(s) to transform")
         return fr
@@ -1573,11 +1490,8 @@ def _apply_rates(fr, cols, models, output_mode):
     made = OrderedDict()
     for c, d, v, nc in zip(cols, data, valid, nulls):
         name = c if output_mode == "replace" else c + "_encoded"
-        made[name] = Column(name, "double", fr.n_rows, dev=d, dev_valid=v, anv_dtype=_lib.ANV_F64, null_count=int(nc))
-    new = OrderedDict((n, made[n] if n in made else fr.column(n)) for n in fr.columns)
-    for n, col in made.items():
-        new.setdefault(n, col)
-    return ColumnFrame(new, fr.n_rows)
+        made[name] = _out_column(fr, c, name, _lib.ANV_F64, d, v, nc)
+    return fr.with_columns(made)
 
 
 def cat_to_num_supervised(spark, idf, list_of_cols="all", drop_cols=[], label_col="label", event_label=1,
@@ -1591,8 +1505,7 @@ def cat_to_num_supervised(spark, idf, list_of_cols="all", drop_cols=[], label_co
     cat_cols = attributeType_segregation(fr)[1]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = cat_cols
-    list_of_cols, drop_cols = _split(list_of_cols), _split(drop_cols)
-    cols = [e for e in dict.fromkeys(list_of_cols) if e not in drop_cols and e != label_col]
+    cols = unique(names(list_of_cols), names(drop_cols) + [label_col])
     if any(x not in cat_cols for x in cols):
         raise TypeError("Invalid input for Column(s)")
     if not cols:
@@ -1668,14 +1581,9 @@ def _apply_outliers(fr, cols, params, output_mode):
     data, _, _ = engine.code_map(fr, cols, [t for _, t in maps], [None] * len(cols))
     made = OrderedDict()
     for c, d, (dic, _) in zip(cols, data, maps):
-        src = fr.column(c)
         name = c if output_mode == "replace" else c + "_outliered"
-        made[name] = Column(name, "string", fr.n_rows, dev=d, dev_valid=src.device()[1], anv_dtype=_lib.ANV_I32,
-                            null_count=src.null_count, dictionary=dic)
-    new = OrderedDict((n, made[n] if n in made else fr.column(n)) for n in fr.columns)
-    for n, col in made.items():
-        new.setdefault(n, col)
-    return ColumnFrame(new, fr.n_rows)
+        made[name] = _out_column(fr, c, name, _lib.ANV_I32, d, sdtype="string", dictionary=dic)
+    return fr.with_columns(made)
 
 
 def outlier_categories(spark, idf, list_of_cols="all", drop_cols=[], coverage=1.0, max_category=50,
@@ -1686,8 +1594,7 @@ def outlier_categories(spark, idf, list_of_cols="all", drop_cols=[], coverage=1.
     cat_cols = attributeType_segregation(fr)[1]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = cat_cols
-    list_of_cols, drop_cols = _split(list_of_cols), _split(drop_cols)
-    cols = [e for e in dict.fromkeys(list_of_cols) if e not in drop_cols]
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(x not in cat_cols for x in cols):
         raise TypeError("Invalid input for Column(s)")
     if not cols:
@@ -1728,7 +1635,7 @@ def cat_to_num_transformer(spark, idf, list_of_cols, drop_cols, method_type, enc
     if len(cat_cols) > 0:
         if isinstance(list_of_cols, str) and list_of_cols == "all":
             list_of_cols = cat_cols
-        list_of_cols = _split(list_of_cols)
+        list_of_cols = names(list_of_cols)
         if any(x not in cat_cols for x in list_of_cols):
             raise TypeError("Invalid input for Column(s)")
         if method_type == "supervised" and label_col is not None:
@@ -1749,7 +1656,5 @@ def _label_to_int(fr, label_col, event_label):
         ev_w, _, _ = label_bitmaps(f, label_col, event_label)
         rows = torch.arange(f.n_rows, device=ev_w.device)
         bit = ((ev_w[rows >> 5] >> (rows & 31).to(torch.int32)) & 1).to(torch.int32)
-        new = OrderedDict((n, f.column(n)) for n in f.columns)
-        new[label_col] = Column(label_col, "int", f.n_rows, dev=bit, anv_dtype=_lib.ANV_I32, null_count=0)
-        return ColumnFrame(new, f.n_rows)
+        return f.with_columns({label_col: Column(label_col, "int", f.n_rows, dev=bit, anv_dtype=_lib.ANV_I32, null_count=0)})
     return _per_chunk(fr, one)

@@ -15,7 +15,7 @@ import pandas as pd
 from .. import profile
 from ..frame import as_frame
 from ..result import ResultFrame
-from ..shared.utils import attributeType_segregation, spark_round
+from ..shared.utils import attributeType_segregation, names, spark_round, unique
 from .validations import check_metric_weightages, check_threshold, compute_si
 
 try:
@@ -23,12 +23,6 @@ try:
 except Exception:  # pragma: no cover
     import logging
     logger = logging.getLogger("anovos_b200")
-
-
-def _names(x):
-    if isinstance(x, str):
-        return [s.strip() for s in x.split("|")]
-    return list(x)
 
 
 def _sample_std(vals):
@@ -63,12 +57,8 @@ def stability_index_computation(spark, idfs, list_of_cols="all", drop_cols=[],
     num_cols = attributeType_segregation(frames[0])[0]
     if isinstance(list_of_cols, str) and list_of_cols == "all":
         list_of_cols = num_cols
-    drop = _names(drop_cols)
-    binary = _names(binary_cols)
-    cols = []
-    for c in _names(list_of_cols):
-        if c not in drop and c not in cols:
-            cols.append(c)
+    binary = names(binary_cols)
+    cols = unique(names(list_of_cols), names(drop_cols))
     if any(c not in num_cols for c in cols) or not cols:
         raise TypeError("Invalid input for Column(s)")
     if any(c not in cols for c in binary):

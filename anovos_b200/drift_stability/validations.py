@@ -15,7 +15,7 @@ import bisect
 import functools
 
 from ..frame import as_frame
-from ..shared.utils import attributeType_segregation
+from ..shared.utils import attributeType_segregation, unique
 
 DISTANCE_METHODS = ("PSI", "JSD", "HD", "KS")
 
@@ -57,7 +57,7 @@ def _resolve_columns(args, kwargs, columns="list_of_cols", target_idx=1, target=
         wanted = num + cat
     wanted = _name_list(wanted, columns)
     dropped = set(_name_list(kwargs.get(drop, []), drop))
-    kept = [c for c in dict.fromkeys(wanted) if c not in dropped]
+    kept = unique(wanted, dropped)
     if not kept:
         raise ValueError("Empty set of columns is given. Columns to select: %s, columns to drop: %s." % (wanted, sorted(dropped)))
     unknown = set(kept) - set(frame.columns)

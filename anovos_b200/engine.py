@@ -804,11 +804,79 @@ def fill_bits(value, anv_dtype) -> int:
     return int(np.array([value], np.int64).view(np.uint64)[0])
 
 
+def _outputs(n_rows, out_dtypes):
+    """One dense output per anv dtype, padded to a multiple of 4 rows so the passes store whole quads."""
+    import torch
+    padded = max((n_rows + 3) // 4 * 4, 4)
+    return [torch.empty(padded, dtype=getattr(torch, _TORCH_OF_ANV[int(od)]), device="cuda") for od in out_dtypes]
+
+
+def _bitmaps(n_rows, flagged):
+    """A zeroed ceil(n_rows/32)-word bitmap per flagged column, None for the others."""
+    import torch
+    n_words = (n_rows + 31) // 32
+    return [torch.zeros(max(n_words, 1), dtype=torch.int32, device="cuda") if f else None for f in flagged]
+
+
+def _bitmap_rows(n_cols, n_rows):
+    """Zeroed bitmaps of n_cols columns as the rows of one [n_cols, ceil(n_rows/32)] int32 tensor."""
+    import torch
+    return torch.zeros((max(n_cols, 1), max((n_rows + 31) // 32, 1)), dtype=torch.int32, device="cuda")
+
+
+def _trimmed(n_rows, outs, valid):
+    """-> (outs, valid) cut to n_rows rows and their ceil(n_rows/32) bitmap words (the allocations are padded)."""
+    n_words = (n_rows + 31) // 32
+    return [t[..., :n_rows] for t in outs], [None if v is None else v[..., :n_words] for v in valid]
+
+
+def _addresses(tensors):
+    """uint64 ndarray of the tensors' device addresses, 0 for None."""
+    return np.array([0 if t is None else t.data_ptr() for t in tensors], np.uint64)
+
+
+def _int64s(dev, n):
+    return _host(dev).view(np.int64)[:n].copy()
+
+
+def _counter_blocks(sizes):
+    """One zeroed device buffer of sum(sizes) 64-bit counters -> (buffer, device address of each block)."""
+    import torch
+    offs = np.cumsum([0] + list(sizes))
+    buf = torch.zeros(max(int(offs[-1]), 1), dtype=torch.int64, device="cuda")
+    return buf, [buf.data_ptr() + 8 * int(o) for o in offs[:-1]]
+
+
+def _read_counter_blocks(buf, sizes):
+    """The blocks of _counter_blocks read back in one copy -> one uint64 ndarray per block."""
+    flat = _host(buf).view(np.uint64)
+    offs = np.cumsum([0] + list(sizes))
+    return [flat[a:b].copy() for a, b in zip(offs[:-1], offs[1:])]
+
+
+def _launch(fn, name, frame, names, args, outs=(), valid=(), null_counts=False):
+    """One launch of an output pass: fn(descriptors of names, *args[, int64 null count per name], len(names), n_rows,
+    stream), the argument order of those entry points.  An ndarray in args is uploaded and passed by its device address,
+    a tensor by its address, None as NULL.  The timer counts one read of the columns plus the rows written to outs and
+    the bitmaps in valid.  -> the null counts as an int64 ndarray if null_counts, else None."""
+    global launch_count
+    held = [_to_dev(a) if isinstance(a, np.ndarray) else a for a in args]      # held until the launch is enqueued
+    desc, keep = frame.descriptors(names)
+    nbytes = input_bytes(frame, names)
+    if timer is not None:
+        nbytes += sum(frame.n_rows * t.element_size() * (t.numel() // t.shape[-1]) for t in outs) + \
+            (frame.n_rows + 31) // 32 * 4 * sum(v is not None for v in valid)
+    nulls = [_dev_bytes(len(names) * 8)] if null_counts else []
+    _call(fn, name, desc.data_ptr(), *[None if a is None else a.data_ptr() for a in held + nulls], len(names),
+          frame.n_rows, _stream(), nbytes=nbytes)
+    launch_count += 1
+    return _int64s(nulls[0], len(names)) if null_counts else None
+
+
 def impute_fill(frame: ColumnFrame, names, out_dtypes, flags, fills):
     """-> list of dense CUDA tensors [n_rows] (one per name, no nulls): anv_impute_fill with per-column output dtype, flags
     (_lib.IMPUTE_*) and fill bits (fill_bits).  One streaming pass over the columns."""
-    global launch_count
-    torch = _lib.require_cuda()
+    _lib.require_cuda()
     L = _lib.lib()
     names = list(names)
     if len(names) > _lib.MAX_LAUNCH_COLS:
@@ -817,39 +885,28 @@ def impute_fill(frame: ColumnFrame, names, out_dtypes, flags, fills):
     if not names:
         return []
     specs = np.zeros(len(names), _IMPUTE_SPEC_DT)
-    outs, ptrs = [], np.zeros(len(names), np.uint64)
-    padded = (frame.n_rows + 3) // 4 * 4
     for i, (n, od, fl, fv) in enumerate(zip(names, out_dtypes, flags, fills)):
         ind = frame.column(n).anv_dtype
         if (ind, od) not in _FILL_PAIRS or (fl & _lib.IMPUTE_NAN_MISSING and ind not in (_lib.ANV_F32, _lib.ANV_F64)):
             raise ValueError("impute_fill: column %r: no fill from dtype %d to %d with flags %d" % (n, ind, od, fl))
         specs[i] = (od, fl, fv)
-        t = torch.empty(max(padded, 4), dtype=getattr(torch, _TORCH_OF_ANV[od]), device="cuda")
-        outs.append(t)
-        ptrs[i] = t.data_ptr()
+    outs = _outputs(frame.n_rows, specs["out_dtype"])
     if frame.n_rows:
-        desc, keep = frame.descriptors(names)
-        dspecs, dptrs = _to_dev(specs), _to_dev(ptrs)
-        nbytes = input_bytes(frame, names)
-        if timer is not None:
-            nbytes += sum(frame.n_rows * t.element_size() for t in outs)
-        _call(L.anv_impute_fill, "anv_impute_fill", desc.data_ptr(), dspecs.data_ptr(), dptrs.data_ptr(), len(names),
-              frame.n_rows, _stream(), nbytes=nbytes)
-        launch_count += 1
-    return [t[:frame.n_rows] for t in outs]
+        _launch(L.anv_impute_fill, "anv_impute_fill", frame, names, (specs, _addresses(outs)), outs)
+    return _trimmed(frame.n_rows, outs, ())[0]
 
 
 def valid_not_nan(frame: ColumnFrame, names):
     """-> (int32 CUDA tensor [n_cols, ceil(n_rows/32)] of "non-null and not NaN" bitmap words, int64 ndarray of NaN counts
     per column).  The Imputer's mean and median are the moments / selection of a view of the column with this bitmap."""
     global launch_count
-    torch = _lib.require_cuda()
+    _lib.require_cuda()
     L = _lib.lib()
     names = list(names)
     if len(names) > _lib.MAX_LAUNCH_COLS:
         return _in_column_blocks(lambda lo, hi: valid_not_nan(frame, names[lo:hi]), len(names))
     n_words = (frame.n_rows + 31) // 32
-    words = torch.zeros((max(len(names), 1), max(n_words, 1)), dtype=torch.int32, device="cuda")
+    words = _bitmap_rows(len(names), frame.n_rows)
     if not names:
         return words[:0, :n_words], np.zeros(0, np.int64)
     desc, keep = frame.descriptors(names)
@@ -857,7 +914,7 @@ def valid_not_nan(frame: ColumnFrame, names):
     _call(L.anv_valid_not_nan, "anv_valid_not_nan", desc.data_ptr(), len(names), frame.n_rows, words.data_ptr(),
           n_nan.data_ptr(), _stream(), nbytes=input_bytes(frame, names))
     launch_count += 1
-    return words[:, :n_words], _host(n_nan).view(np.int64)[:len(names)].copy()
+    return words[:, :n_words], _int64s(n_nan, len(names))
 
 
 # ---- scaling -------------------------------------------------------------------------------------
@@ -870,40 +927,26 @@ def scale_columns(frame: ColumnFrame, names, specs):
     """anv_scale_columns: specs = one (mode, out anv dtype, flags, a, b, c) per name (_lib.SCALE_*).
     -> (list of CUDA tensors [n_rows] in the output dtype, list of int32 bitmap tensors [ceil(n_rows/32)] for the
     NAN_TO_NULL columns and None for the others (which keep the source's validity), int64 ndarray of null counts)."""
-    global launch_count
-    torch = _lib.require_cuda()
+    _lib.require_cuda()
     L = _lib.lib()
     names, specs = list(names), list(specs)
     if len(names) > _lib.MAX_LAUNCH_COLS:
         return _in_column_blocks(lambda lo, hi: scale_columns(frame, names[lo:hi], specs[lo:hi]), len(names))
     sp = np.zeros(len(names), _SCALE_SPEC_DT)
-    outs, ptrs = [], np.zeros(len(names), np.uint64)
-    padded = (frame.n_rows + 3) // 4 * 4
     for i, (n, (mode, od, fl, a, b, c)) in enumerate(zip(names, specs)):
         if mode not in (_lib.SCALE_DIV, _lib.SCALE_AFFINE, _lib.SCALE_CONST) or od not in (_lib.ANV_F32, _lib.ANV_F64) \
                 or frame.column(n).anv_dtype not in _NP_OF_ANV or fl & ~_lib.SCALE_NAN_TO_NULL:
             raise ValueError("scale_columns: column %r: no scale mode %r to dtype %r with flags %r" % (n, mode, od, fl))
         sp[i] = (mode, od, fl, 0, a, b, c)
-        t = torch.empty(max(padded, 4), dtype=getattr(torch, _TORCH_OF_ANV[od]), device="cuda")
-        outs.append(t)
-        ptrs[i] = t.data_ptr()
-    n_words = (frame.n_rows + 31) // 32
+    outs = _outputs(frame.n_rows, sp["out_dtype"])
     flagged = [bool(s[2] & _lib.SCALE_NAN_TO_NULL) for s in specs]
-    words = torch.zeros((max(len(names), 1), max(n_words, 1)), dtype=torch.int32, device="cuda") if any(flagged) else None
-    if not names or not frame.n_rows:
-        return [t[:frame.n_rows] for t in outs], [None if words is None else words[i, :n_words] if f else None
-                                                  for i, f in enumerate(flagged)], np.zeros(len(names), np.int64)
-    nulls = _dev_bytes(len(names) * 8)
-    desc, keep = frame.descriptors(names)
-    nbytes = input_bytes(frame, names)
-    if timer is not None:
-        nbytes += sum(frame.n_rows * t.element_size() + (n_words * 4 if f else 0) for t, f in zip(outs, flagged))
-    dspecs, dptrs = _to_dev(sp), _to_dev(ptrs)          # held until the launch is enqueued
-    _call(L.anv_scale_columns, "anv_scale_columns", desc.data_ptr(), dspecs.data_ptr(), dptrs.data_ptr(),
-          None if words is None else words.data_ptr(), nulls.data_ptr(), len(names), frame.n_rows, _stream(), nbytes=nbytes)
-    launch_count += 1
-    valid = [words[i, :n_words] if f else None for i, f in enumerate(flagged)]
-    return [t[:frame.n_rows] for t in outs], valid, _host(nulls).view(np.int64)[:len(names)].copy()
+    words = _bitmap_rows(len(names), frame.n_rows) if any(flagged) else None
+    valid = [words[i] if f else None for i, f in enumerate(flagged)]
+    nulls = np.zeros(len(names), np.int64)
+    if names and frame.n_rows:
+        nulls = _launch(L.anv_scale_columns, "anv_scale_columns", frame, names, (sp, _addresses(outs), words), outs, valid,
+                        null_counts=True)
+    return (*_trimmed(frame.n_rows, outs, valid), nulls)
 
 
 # ---- feature transformation ----------------------------------------------------------------------
@@ -929,40 +972,25 @@ def transform_columns(frame: ColumnFrame, names, specs):
     -> (list of CUDA tensors [n_rows] in the output dtype, list of int32 bitmap tensors [ceil(n_rows/32)] for the ops that
     make nulls (_lib.TF_MAKES_NULLS) and None for the others (which keep the source's validity), int64 ndarray of null
     counts)."""
-    global launch_count
-    torch = _lib.require_cuda()
+    _lib.require_cuda()
     L = _lib.lib()
     names, specs = list(names), list(specs)
     if len(names) > _lib.MAX_LAUNCH_COLS:
         return _in_column_blocks(lambda lo, hi: transform_columns(frame, names[lo:hi], specs[lo:hi]), len(names))
     sp = np.zeros(len(names), _TRANSFORM_SPEC_DT)
-    outs, ptrs = [], np.zeros(len(names), np.uint64)
-    padded = (frame.n_rows + 3) // 4 * 4
     for i, (n, (op, od, k, a)) in enumerate(zip(names, specs)):
         ind = frame.column(n).anv_dtype
         if ind not in _NP_OF_ANV or not transform_spec_ok(op, ind, od, k):
             raise ValueError("transform_columns: column %r: no op %r from dtype %r to %r with n = %r" % (n, op, ind, od, k))
         sp[i] = (op, od, k, a)
-        t = torch.empty(max(padded, 4), dtype=getattr(torch, _TORCH_OF_ANV[od]), device="cuda")
-        outs.append(t)
-        ptrs[i] = t.data_ptr()
-    n_words = (frame.n_rows + 31) // 32
+    outs = _outputs(frame.n_rows, sp["out_dtype"])
     flagged = [s[0] in _lib.TF_MAKES_NULLS for s in specs]
-    valid = [torch.zeros(max(n_words, 1), dtype=torch.int32, device="cuda")[:n_words] if f else None for f in flagged]
-    vptrs = np.array([0 if v is None else v.data_ptr() for v in valid], np.uint64)
-    if not names or not frame.n_rows:
-        return [t[:frame.n_rows] for t in outs], valid, np.zeros(len(names), np.int64)
-    nulls = _dev_bytes(len(names) * 8)
-    desc, keep = frame.descriptors(names)
-    nbytes = input_bytes(frame, names)
-    if timer is not None:
-        nbytes += sum(frame.n_rows * t.element_size() + (n_words * 4 if f else 0) for t, f in zip(outs, flagged))
-    dspecs, dptrs = _to_dev(sp), _to_dev(ptrs)          # held until the launch is enqueued
-    dvptrs = _to_dev(vptrs) if any(flagged) else None
-    _call(L.anv_transform_columns, "anv_transform_columns", desc.data_ptr(), dspecs.data_ptr(), dptrs.data_ptr(),
-          None if dvptrs is None else dvptrs.data_ptr(), nulls.data_ptr(), len(names), frame.n_rows, _stream(), nbytes=nbytes)
-    launch_count += 1
-    return [t[:frame.n_rows] for t in outs], valid, _host(nulls).view(np.int64)[:len(names)].copy()
+    valid = _bitmaps(frame.n_rows, flagged)
+    nulls = np.zeros(len(names), np.int64)
+    if names and frame.n_rows:
+        nulls = _launch(L.anv_transform_columns, "anv_transform_columns", frame, names,
+                        (sp, _addresses(outs), _addresses(valid) if any(flagged) else None), outs, valid, null_counts=True)
+    return (*_trimmed(frame.n_rows, outs, valid), nulls)
 
 
 def ks_candidates(frame: ColumnFrame, name, lambdas, n_null):
@@ -1007,15 +1035,12 @@ def code_map(frame: ColumnFrame, names, tables, entry_valid):
     slot); entry_valid = per name, a bool array of the same length or None.
     -> (list of CUDA tensors [n_rows] in the table's dtype, list of int32 bitmap tensors [ceil(n_rows/32)] for the names
     with entry_valid and None for the others (which keep the source's validity), int64 ndarray of null counts)."""
-    global launch_count
-    torch = _lib.require_cuda()
+    _lib.require_cuda()
     L = _lib.lib()
     names, tables, entry_valid = list(names), list(tables), list(entry_valid)
     if len(names) > _lib.MAX_LAUNCH_COLS:
         return _in_column_blocks(lambda lo, hi: code_map(frame, names[lo:hi], tables[lo:hi], entry_valid[lo:hi]), len(names))
-    n_words = (frame.n_rows + 31) // 32
-    padded = max((frame.n_rows + 3) // 4 * 4, 4)
-    host, outs, valid = [], [], []
+    host, ods, flagged = [], [], []
     for n, t, ev in zip(names, tables, entry_valid):
         col = frame.column(n)
         size = len(col.dictionary) if col.dictionary is not None else -1
@@ -1025,29 +1050,18 @@ def code_map(frame: ColumnFrame, names, tables, entry_valid):
         host.append(t)
         if ev is not None:
             host.append(np.packbits(np.asarray(ev, bool), bitorder="little"))
-        outs.append(torch.empty(padded, dtype=torch.int32 if t.dtype == np.int32 else torch.float64, device="cuda"))
-        valid.append(torch.zeros(max(n_words, 1), dtype=torch.int32, device="cuda") if ev is not None else None)
-    if not names or not frame.n_rows:
-        return [t[:frame.n_rows] for t in outs], [None if v is None else v[:n_words] for v in valid], \
-            np.zeros(len(names), np.int64)
-    buf, addr = _tables_to_dev(host)
-    sp = np.zeros(len(names), _CODE_MAP_SPEC_DT)
-    a = iter(addr)
-    for i, (n, t, ev) in enumerate(zip(names, tables, entry_valid)):
-        od = _lib.ANV_I32 if t.dtype == np.int32 else _lib.ANV_F64
-        sp[i] = (len(t) - 1, od, next(a), next(a) if ev is not None else 0, outs[i].data_ptr(),
-                 valid[i].data_ptr() if valid[i] is not None else 0)
-    nulls = _dev_bytes(len(names) * 8)
-    desc, keep = frame.descriptors(names)
-    nbytes = input_bytes(frame, names)
-    if timer is not None:
-        nbytes += sum(frame.n_rows * t.element_size() + (n_words * 4 if v is not None else 0) for t, v in zip(outs, valid))
-    dspecs = _to_dev(sp)                                # held until the launch is enqueued
-    _call(L.anv_code_map, "anv_code_map", desc.data_ptr(), dspecs.data_ptr(), nulls.data_ptr(), len(names), frame.n_rows,
-          _stream(), nbytes=nbytes)
-    launch_count += 1
-    return [t[:frame.n_rows] for t in outs], [None if v is None else v[:n_words] for v in valid], \
-        _host(nulls).view(np.int64)[:len(names)].copy()
+        ods.append(_lib.ANV_I32 if t.dtype == np.int32 else _lib.ANV_F64)
+        flagged.append(ev is not None)
+    outs, valid = _outputs(frame.n_rows, ods), _bitmaps(frame.n_rows, flagged)
+    nulls = np.zeros(len(names), np.int64)
+    if names and frame.n_rows:
+        buf, addr = _tables_to_dev(host)
+        sp = np.zeros(len(names), _CODE_MAP_SPEC_DT)
+        a, out_addr, valid_addr = iter(addr), _addresses(outs), _addresses(valid)
+        for i, (t, f) in enumerate(zip(tables, flagged)):
+            sp[i] = (len(t) - 1, ods[i], next(a), next(a) if f else 0, out_addr[i], valid_addr[i])
+        nulls = _launch(L.anv_code_map, "anv_code_map", frame, names, (sp,), outs, valid, null_counts=True)
+    return (*_trimmed(frame.n_rows, outs, valid), nulls)
 
 
 def one_hot_stride(n_rows):
@@ -1059,7 +1073,6 @@ def one_hot(frame: ColumnFrame, names, indexes, ks):
     """anv_one_hot: indexes = per name, a host int32 array of len(dictionary) + 1 entries (the last is the null slot) in
     [0, k); ks = output columns per name.  -> list of int32 CUDA tensors [k, n_rows], row j = (index == j), each row a
     16-byte aligned view of one [k, one_hot_stride(n_rows)] allocation."""
-    global launch_count
     torch = _lib.require_cuda()
     L = _lib.lib()
     names, indexes, ks = list(names), list(indexes), [int(k) for k in ks]
@@ -1074,21 +1087,13 @@ def one_hot(frame: ColumnFrame, names, indexes, ks):
             raise ValueError("one_hot: column %r needs a string column, an int32 index of its dictionary size + 1 and k >= 1"
                              % n)
         outs.append(torch.empty((k, stride), dtype=torch.int32, device="cuda"))
-    if not names or not frame.n_rows:
-        return [o[:, :frame.n_rows] for o in outs]
-    buf, addr = _tables_to_dev(indexes)
-    sp = np.zeros(len(names), _ONE_HOT_SPEC_DT)
-    for i in range(len(names)):
-        sp[i] = (len(indexes[i]) - 1, ks[i], addr[i], outs[i].data_ptr(), stride)
-    desc, keep = frame.descriptors(names)
-    nbytes = input_bytes(frame, names)
-    if timer is not None:
-        nbytes += sum(frame.n_rows * 4 * k for k in ks)
-    dspecs = _to_dev(sp)
-    _call(L.anv_one_hot, "anv_one_hot", desc.data_ptr(), dspecs.data_ptr(), len(names), frame.n_rows, _stream(),
-          nbytes=nbytes)
-    launch_count += 1
-    return [o[:, :frame.n_rows] for o in outs]
+    if names and frame.n_rows:
+        buf, addr = _tables_to_dev(indexes)
+        sp = np.zeros(len(names), _ONE_HOT_SPEC_DT)
+        for i in range(len(names)):
+            sp[i] = (len(indexes[i]) - 1, ks[i], addr[i], outs[i].data_ptr(), stride)
+        _launch(L.anv_one_hot, "anv_one_hot", frame, names, (sp,), outs)
+    return _trimmed(frame.n_rows, outs, ())[0]
 
 
 # ---- table membership (invalidEntries_detection) --------------------------------------------------
@@ -1112,7 +1117,6 @@ def flag_members(frame: ColumnFrame, names, tables, want_bitmap):
             raise ValueError("flag_members: a row-partitioned frame counts only; map_chunks gives the treated chunks")
         return frame.flag_members(list(names), list(tables)), [None] * len(list(names))
     from .shared.invalid_rules import ordered_keys
-    global launch_count
     torch = _lib.require_cuda()
     L = _lib.lib()
     names, tables = list(names), list(tables)
@@ -1137,26 +1141,17 @@ def flag_members(frame: ColumnFrame, names, tables, want_bitmap):
     if want_bitmap:
         for i in launch:
             valid[i] = torch.empty(max(n_words, 1), dtype=torch.int32, device="cuda")
-    offs = np.cumsum([0] + [len(keys[i]) for i in launch])
-    dcounts = torch.zeros(max(int(offs[-1]), 1), dtype=torch.int64, device="cuda")
+    sizes = [len(keys[i]) for i in launch]
+    dcounts, count_addr = _counter_blocks(sizes)
     buf, addr = _tables_to_dev([keys[i] for i in launch])
     sp = np.zeros(len(launch), _FLAG_SPEC_DT)
     for j, i in enumerate(launch):
-        sp[j] = (addr[j], len(keys[i]), dcounts.data_ptr() + 8 * int(offs[j]),
-                 valid[i].data_ptr() if valid[i] is not None else 0)
-    lnames = [names[i] for i in launch]
-    desc, keep = frame.descriptors(lnames)
-    nbytes = input_bytes(frame, lnames)
-    if timer is not None and want_bitmap:
-        nbytes += len(launch) * n_words * 4
-    dspecs = _to_dev(sp)                                # held until the launch is enqueued
-    _call(L.anv_flag_members, "anv_flag_members", desc.data_ptr(), dspecs.data_ptr(), len(launch), frame.n_rows, _stream(),
-          nbytes=nbytes)
-    launch_count += 1
-    flat = _host(dcounts).view(np.uint64)
-    for j, i in enumerate(launch):
-        counts[i] = flat[offs[j]:offs[j + 1]].copy()
-    return counts, [None if v is None else v[:n_words] for v in valid]
+        sp[j] = (addr[j], len(keys[i]), count_addr[j], valid[i].data_ptr() if valid[i] is not None else 0)
+    _launch(L.anv_flag_members, "anv_flag_members", frame, [names[i] for i in launch], (sp,),
+            valid=[valid[i] for i in launch])
+    for i, c in zip(launch, _read_counter_blocks(dcounts, sizes)):
+        counts[i] = c
+    return counts, _trimmed(frame.n_rows, (), valid)[1]
 
 
 # ---- label-class histogram (monotonic_binning) ----------------------------------------------------
@@ -1187,8 +1182,7 @@ def class_hist(frame: ColumnFrame, names, thresholds, label_col, event_label):
 
 
 def _class_hist_words(frame, names, thresholds, ev_words, nev_words):
-    global launch_count
-    torch = _lib.require_cuda()
+    _lib.require_cuda()
     L = _lib.lib()
     if len(names) > _lib.MAX_LAUNCH_COLS:
         return _in_column_blocks(lambda lo, hi: _class_hist_words(frame, names[lo:hi], thresholds[lo:hi], ev_words,
@@ -1202,18 +1196,13 @@ def _class_hist_words(frame, names, thresholds, ev_words, nev_words):
                 or (len(t) > 1 and not bool(np.all(t[1:] > t[:-1]))):
             raise ValueError("class_hist: column %r needs at most %d distinct ascending %s thresholds" % (n, max_thr, want))
         thr.append(t)
-    offs = np.cumsum([0] + [class_hist_counters(len(t)) for t in thr])
+    sizes = [class_hist_counters(len(t)) for t in thr]
     if not names or not frame.n_rows:
-        return [np.zeros(int(offs[i + 1] - offs[i]), np.uint64) for i in range(len(names))]
-    dcounts = torch.zeros(int(offs[-1]), dtype=torch.int64, device="cuda")
+        return [np.zeros(k, np.uint64) for k in sizes]
+    dcounts, count_addr = _counter_blocks(sizes)
     buf, addr = _tables_to_dev(thr)
     sp = np.zeros(len(names), _CLASS_HIST_SPEC_DT)
     for i, t in enumerate(thr):
-        sp[i] = (addr[i], len(t), 0, dcounts.data_ptr() + 8 * int(offs[i]))
-    desc, keep = frame.descriptors(names)
-    dspecs = _to_dev(sp)                                # held until the launch is enqueued
-    _call(L.anv_class_hist, "anv_class_hist", desc.data_ptr(), dspecs.data_ptr(), ev_words.data_ptr(), nev_words.data_ptr(),
-          len(names), frame.n_rows, _stream(), nbytes=input_bytes(frame, names))
-    launch_count += 1
-    flat = _host(dcounts).view(np.uint64)
-    return [flat[offs[i]:offs[i + 1]].copy() for i in range(len(names))]
+        sp[i] = (addr[i], len(t), 0, count_addr[i])
+    _launch(L.anv_class_hist, "anv_class_hist", frame, names, (sp, ev_words, nev_words))
+    return _read_counter_blocks(dcounts, sizes)

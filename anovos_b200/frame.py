@@ -282,6 +282,14 @@ class ColumnFrame:
         names = set(names[0]) if len(names) == 1 and isinstance(names[0], (list, tuple, set)) else set(names)
         return ColumnFrame(OrderedDict((n, c) for n, c in self._cols.items() if n not in names), self.n_rows)
 
+    def with_columns(self, cols, drop=()) -> "ColumnFrame":
+        """The frame without `drop`, then with `cols` (an ordered name -> Column mapping): a name the frame still has is
+        replaced in place, a new one is appended in the order of `cols` (Spark's withColumn, one call per column)."""
+        drop = set(drop)
+        out = OrderedDict((n, c) for n, c in self._cols.items() if n not in drop)
+        out.update(cols)
+        return ColumnFrame(out, self.n_rows)
+
     def valid_mask(self, name):
         """bool CUDA tensor [n_rows]: True where column `name` is non-null (frame transforms only)."""
         torch = _lib.require_cuda()

@@ -12,6 +12,20 @@ _QUANT = {4: Decimal("0.0001")}
 _WIDE = Context(prec=340)
 
 
+def names(x):
+    """A column-list argument as a list: a string is the reference's "a|b|c" form, anything else an iterable of names."""
+    if isinstance(x, str):
+        return [s.strip() for s in x.split("|")]
+    return list(x)
+
+
+def unique(cols, drop):
+    """cols without repeats and without the names in drop, in first-seen order (the reference's list(set(...)) has no
+    order); drop is looked up in a set so that wide frames stay linear."""
+    drop = set(drop)
+    return [c for c in dict.fromkeys(cols) if c not in drop]
+
+
 def attributeType_segregation(idf):
     """-> (num_cols, cat_cols, other_cols) by Spark dtype string (shared/utils.py:64-72)."""
     fr = as_frame(idf)

@@ -199,3 +199,17 @@ def test_folded_bin_guess_stays_within_one_bin_of_the_exact_slot(seed):
                 assert r + (0 if x <= s_r else 1) == b + 1
                 checked += 1
     assert checked > 20000
+
+
+def test_with_columns_replaces_in_place_appends_in_order_and_drop_moves_to_the_end():
+    from anovos_b200.frame import Column, ColumnFrame
+    fr = ColumnFrame.from_pandas(pd.DataFrame({"a": [1, 2], "b": [3, 4], "c": [5, 6]}))
+
+    def col(name):
+        return Column(name, "int", 2, host=np.array([7, 8], np.int32))
+    made = {"z": col("z"), "b": col("b"), "y": col("y")}
+    out = fr.with_columns(made)
+    assert out.columns == ["a", "b", "c", "z", "y"] and out.n_rows == 2
+    assert out.column("b") is made["b"] and out.column("a") is fr.column("a")
+    assert fr.columns == ["a", "b", "c"] and fr.column("b") is not made["b"]          # the input frame is unchanged
+    assert fr.with_columns(made, drop=["b", "a"]).columns == ["c", "z", "b", "y"]
